@@ -1,17 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- ZigMa denoiser hot path on B200 (BASELINE.json metric).
+"""bench.py -- ZigMa denoiser hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one denoiser evaluation (ZigMa.forward at the per-GPU batch of the workload, bf16, synthetic weights /
 latents) followed by the Euler update of the flow-matching sampler (transport/integrators.py:105-123).  The default
 workload is BASELINE.json configs[1] (zigzag8_b1, bs=64 per GPU); --config selects one of the other BASELINE
 configs, and the default run also measures them (a few evaluations each) into the `configs` block of its line.
-Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for how every field is obtained.
+Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for how every field is obtained.  Nothing is written to the source
+tree.  --dump-outputs DIR stores what the timed K-step loop returned (the gathered final latents) as DIR/latents.npy (float32):
+weights, noise and time grid are seeded, so two builds run with the same arguments can be compared output for output.
 
 --impl reference: the reference's own implementation of the path on the HOST cores (no GPU, no import of the
-product package): the pinned CPU restatement in oracle/ (the reference is Python and cannot travel to the GPU box),
+product package): the pinned CPU restatement in oracle/ (the reference itself is not part of this repository),
 same workload and batch, unscaled.
 """
 import argparse
@@ -28,7 +30,8 @@ sys.path.insert(0, ROOT)
 NUM_GRID = 50           # linspace(0, 1, 50): the sampler's time grid (49 evaluations per sample)
 
 # BASELINE.json `configs` (configs[0] is the CPU correctness case: tests/).  Per-GPU batches: configs 3 / 4 are quoted as
-# bs 256 / 128 "sharded across 8xB200" = 32 / 16 per GPU; model hyper-parameters from /root/reference/config/model/*.yaml.
+# bs 256 / 128 sharded across 8 GPUs = 32 / 16 per GPU (the activations of one evaluation stay under 10 GB, well inside the 80 GB
+# of an H100); model hyper-parameters from the reference's config/model/*.yaml.
 WORKLOADS = {
     "zigzag8_b1": dict(
         cfg=dict(in_channels=4, embed_dim=640, depth=18, img_dim=32, patch_size=1, scan_type="zigzagN8", use_pe=2),
@@ -60,14 +63,15 @@ def scan_algorithmic_bytes(Bt, E, L, N, s):
     return 4 * s * Bt * E * L + 2 * s * Bt * N * L + 4 * (E * N + 2 * E)
 
 
-def scan_mufu_floor_ms(Bt, E, L, N, sm_mhz=1965.0, n_sm=148):
+def scan_mufu_floor_ms(Bt, E, L, N, sm_mhz=1980.0, n_sm=132):
     """Compute ceiling of the scan that sits ABOVE its HBM time: N exp2 per (b, e, l) for the state decays plus 4 for
-    softplus (ex2 + lg2) and SiLU (ex2 + rcp) on the 16-lane/SM MUFU pipe (DESIGN.md 4.1)."""
+    softplus (ex2 + lg2) and SiLU (ex2 + rcp) on the 16-lane/SM MUFU pipe (DESIGN.md 4.1).  Defaults: H100 SXM, 132 SMs at the
+    1980 MHz maximum SM clock of the data sheet (a power-limited card runs lower, so the real floor is higher)."""
     return (N + 4) * Bt * E * L / (n_sm * 16 * sm_mhz * 1e6) * 1e3
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -92,6 +96,7 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm = sorted(float(r[1]) for r in self.rows if len(r) >= 9 and r[1].replace(".", "").isdigit())
         mx = [float(r[2]) for r in self.rows if len(r) >= 9 and r[2].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -105,7 +110,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json, copy kernel, burst)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s); not a measured figure"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -145,7 +150,7 @@ def cpu_reference_eval(name, bs, state=None, nthreads=None):
 
 def run_reference(args, rank):
     """--impl reference: the reference's own (CPU) implementation of the path, timed on the host cores -- the pinned CPU
-    restatement in oracle/ (kind 'port': the Python reference cannot travel to the GPU box).  SAME workload and batch as
+    restatement in oracle/ (kind 'port').  SAME workload and batch as
     the `ours` arm, unscaled; the number of timed evaluations is capped so that the run ends within a few minutes."""
     if rank != 0:
         return          # one host: rank 0 alone runs the CPU arm
@@ -153,7 +158,7 @@ def run_reference(args, rank):
     wl = WORKLOADS[name]
     bs = args.bs or wl["bs"]
     cores = os.cpu_count() or 1
-    threads = int(os.environ.get("ZIGMA_REF_THREADS", "0")) or min(cores, 32)      # torch intra-op threads; measured on the 128-core box: 55 s / evaluation with 32, 112 s with 128 (the C scan uses OpenMP's default: all cores)
+    threads = int(os.environ.get("ZIGMA_REF_THREADS", "0")) or min(cores, 32)      # torch intra-op threads: more than 32 slowed the GEMMs of this path down (the C scan uses OpenMP's default: all cores)
     state = cpu_reference_setup(name)
     cpu_reference_eval(name, 1, state, threads)                  # page in / build the C oracle (not timed)
     budget_s = float(os.environ.get("ZIGMA_REF_BUDGET_S", "150"))
@@ -184,7 +189,7 @@ def run_reference(args, rank):
 # ours
 # ------------------------------------------------------------------------------------------------
 def reference_cuda_numbers(name, bs, n_iter=3):
-    """The reference's vendored CUDA kernels (oracle/_ref, built from the unmodified sources for sm_100a) on this GPU:
+    """The reference's vendored CUDA kernels (oracle/_ref, built from the unmodified sources for sm_90a) on this GPU:
     (a) selective_scan_cuda.fwd and causal_conv1d_fwd at the layer shape of the workload in the reference's own layout,
     (b) one denoiser evaluation through the reference's (restated) PyTorch glue around those kernels.  Returns None when
     oracle/_ref is absent.  (Runs in the `ours` arm only: it needs the GPU.)"""
@@ -244,7 +249,7 @@ def reference_cuda_numbers(name, bs, n_iter=3):
     finally:
         zo.BACKEND = {}
     out.update({"denoiser_eval_ms": ms, "tokens_per_s": bs * wl["tokens"] / (ms * 1e-3), "bs": bs, "dtype": "bf16",
-                "what": "reference dis_mamba/dis_causal_conv1d CUDA kernels (sm_100a build of the unmodified sources) + the reference's PyTorch glue (restated), eager"})
+                "what": "reference dis_mamba/dis_causal_conv1d CUDA kernels (sm_90a build of the unmodified sources) + the reference's PyTorch glue (restated), eager"})
     return out
 
 
@@ -289,34 +294,25 @@ def scan_roofline(name, bs, dev, step_ms=None, depth=None):
         s0, s1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s0.record()
         for _ in range(n_it):
-            call()      # working set 4 x (sb L E 2 B) >> 126 MB L2 at every benchmark shape: each launch streams from HBM
+            call()      # working set 4 x (sb L E 2 B) >> 50 MB L2 at every benchmark shape: each launch streams from HBM
         s1.record()
         torch.cuda.synchronize()
         kms = s0.elapsed_time(s1) / n_it
         abytes = scan_algorithmic_bytes(sb, E, L, N, 2)
         ach = abytes / (kms * 1e-3) / 1e9
-        floor = scan_mufu_floor_ms(sb, E, L, N)
+        floor = scan_mufu_floor_ms(sb, E, L, N, n_sm=torch.cuda.get_device_properties(dev).multi_processor_count)
         from zigma_b200 import _lib as _zl
         res.append({"shape": f"{kind}: batch {sb} x dim {E} x seqlen {L}", "kernel": _zl.last_scan_kernel(), "ms_per_launch": kms, "algorithmic_bytes": abytes, "achieved": ach,
                     "frac": ach / peak, "hbm_floor_ms": abytes / (peak * 1e9) * 1e3, "compute_floor_ms": floor, "frac_of_compute_floor": floor / kms})
         del xz, xc, dl, xdbl, outb
     r0 = res[0]
     kname = res[0]["kernel"]
-    traffic, tsrc = None, None
-    if name == DEFAULT:     # DRAM bytes of one launch from this round's ncu capture of the kernel that actually ran
-        for fn in ("r02b_scan_fwd_traffic.json", "r02_scan_fwd_traffic.json"):
-            tp = os.path.join(ROOT, "profiles", fn)
-            if os.path.exists(tp):
-                tj = json.load(open(tp))
-                if tj.get("kernel", "zg::scan_fwd_tma_kernel") in kname:
-                    traffic, tsrc = tj.get("dram_bytes_per_launch"), tj.get("source")
-                    break
     roof = {"bound": "hbm", "kernel": kname + " <bf16>: dstate 16, token-major, z gathered through the zigzag table",
-            "achieved": r0["achieved"], "peak": peak, "unit": "GB/s", "frac": r0["frac"], "traffic": traffic, "traffic_source": tsrc,
+            "achieved": r0["achieved"], "peak": peak, "unit": "GB/s", "frac": r0["frac"],
             "peak_source": how, "ms_per_launch": r0["ms_per_launch"], "algorithmic_bytes": r0["algorithmic_bytes"],
             "hbm_floor_ms": r0["hbm_floor_ms"],
             "compute_floor_ms": r0["compute_floor_ms"], "frac_of_compute_floor": r0["frac_of_compute_floor"],
-            "compute_floor_what": "MUFU pipe: (16 + 4) ex2/lg2/rcp per (b, e, l) at 16 lanes/SM/clk, 148 SMs, 1965 MHz -- the scan is compute-bound ABOVE its HBM time, so frac (of the HBM roofline) cannot exceed hbm_floor_ms / compute_floor_ms",
+            "compute_floor_what": "MUFU pipe: (16 + 4) ex2/lg2/rcp per (b, e, l) at 16 lanes/SM/clk, this device's SM count, 1980 MHz (H100 SXM data-sheet maximum) -- the scan is compute-bound ABOVE its HBM time, so frac (of the HBM roofline) cannot exceed hbm_floor_ms / compute_floor_ms",
             "shapes": res}
     if step_ms and depth:
         per_layer = sum(r["ms_per_launch"] for r in res) if name != "ucf101_sst" else None
@@ -348,7 +344,7 @@ def other_kernel_rooflines(name, bs, dev):
     dtype = torch.bfloat16
     hbm, _ = measured_peaks()
     pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    tf_peak = float(pk.get("bf16_tflops", 1666.9))          # burst figure: each kernel is timed alone
+    tf_peak = float(pk.get("bf16_tflops", 989.0))           # fallback: H100 SXM data sheet, dense bf16 at 700 W (not a measured figure)
 
     def timeit(fn, n=20):
         for _ in range(3):
@@ -456,7 +452,7 @@ def run_workload(name, bs, K, W, dev, world, rank, use_graph=True, with_e2e=True
             clocks.start()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
-        torch.cuda.profiler.start()     # no-op unless run under `ncu --profile-from-start off`
+        torch.cuda.profiler.start()     # no-op unless run under a profiler that waits for it
         e0.record()
         x = sample(z0)                  # exactly K steps
         full = gather_latents(x, bs * world, world)      # the single collective of the sampling job
@@ -470,7 +466,7 @@ def run_workload(name, bs, K, W, dev, world, rank, use_graph=True, with_e2e=True
             dist.all_reduce(tm, op=dist.ReduceOp.MAX)
             ms = tm.item()
         assert torch.isfinite(full.float()).all()
-        res = {"ms": ms, "ms_per_step": ms / K, "per_eval": per_eval, "clocks": clk, "bs": bs, "warm_steps": n_warm * K,
+        res = {"ms": ms, "ms_per_step": ms / K, "per_eval": per_eval, "final_latents": full.float().cpu() if rank == 0 else None, "clocks": clk, "bs": bs, "warm_steps": n_warm * K,
                "tokens_per_s": bs * world * wl["tokens"] * K / (ms * 1e-3)}
 
         if with_e2e:
@@ -518,9 +514,11 @@ def main():
     ap.add_argument("--bs", type=int, default=0, help="batch per GPU (default: the workload's BASELINE batch)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ref-cuda", action="store_true")
-    ap.add_argument("--no-graph", action="store_true", help="launch kernels eagerly (for ncu launch lists)")
+    ap.add_argument("--no-graph", action="store_true", help="launch kernels eagerly (for per-kernel launch lists)")
     ap.add_argument("--no-train", action="store_true", help="skip the forward+backward (training step) side measurement")
     ap.add_argument("--no-configs", action="store_true", help="skip the side measurements of the other BASELINE configs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result of the timed K-step loop (gathered final latents) to DIR/latents.npy as float32")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -543,6 +541,13 @@ def main():
     bs = args.bs or wl["bs"]
 
     main_res = run_workload(name, bs, K, W, dev, world, rank, use_graph=not args.no_graph)
+    final_latents = main_res.pop("final_latents")
+    if args.dump_outputs and rank == 0:
+        # (global_batch, *latent) float32: 1 MB at the default workload, 16 MB per GPU at the largest one
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), final_latents.numpy())
+    del final_latents
     roof = scan_roofline(name, bs, dev, main_res["ms_per_step"], wl["cfg"]["depth"]) if rank == 0 else None
     if world > 1:
         dist.barrier()
@@ -562,9 +567,9 @@ def main():
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": f"{wl['desc']}, bs={bs}/GPU, fixed-grid Euler (linspace(0,1,50))",
                    "global_batch": bs * world, "seq_len": wl["tokens"], "parallelism": f"dp{world}",
-                   "l2_policy": "no flush: per-step working set (xz alone >= 335 MB per layer) >> 126 MB L2",
+                   "l2_policy": "no flush: per-step working set (xz alone >= 335 MB per layer) >> 50 MB L2",
                    "denoiser_steps_per_s": K / (ms * 1e-3), "cuda_graph": "one graph replay = the whole K-step Euler loop" if not args.no_graph else False,
-                   "gemm": "hand-written tcgen05 (zg_gemm_bf16_tn)" if os.environ.get("ZIGMA_TCGEN05", "1") == "1" else "library (cuBLAS)",
+                   "gemm": "hand-written wgmma (zg_gemm_bf16_tn)" if os.environ.get("ZIGMA_TCGEN05", "1") == "1" else "library (cuBLAS)",
                    "collective": "one all_gather of final latents, inside the timed region"},
         "clocks": main_res["clocks"],
         "e2e": main_res.get("e2e"),
@@ -589,6 +594,7 @@ def main():
             try:
                 obs = WORKLOADS[other]["bs"]
                 r = run_workload(other, obs, 5, 3, dev, 1, 0, use_graph=not args.no_graph, with_e2e=False)
+                del r["final_latents"]
                 ro = scan_roofline(other, obs, dev, r["ms_per_step"], WORKLOADS[other]["cfg"]["depth"])
                 ent = {"workload": WORKLOADS[other]["desc"], "bs_per_gpu": obs, "seq_len": WORKLOADS[other]["tokens"], "steps": 5,
                        "ms_per_eval": r["ms_per_step"], "tokens_per_s_per_gpu": r["tokens_per_s"], "gpu_launches_per_eval": r["per_eval"],

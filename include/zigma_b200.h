@@ -1,5 +1,5 @@
 /*
- * zigma_b200 -- C-ABI of the B200 (sm_100a) kernels for the ZigMa denoiser hot path.
+ * zigma_b200 -- C-ABI of the H100 (sm_90a) kernels for the ZigMa denoiser hot path.
  *
  * This header is the drop-in boundary.  Every entry point replaces one native interface of the
  * reference (CompVis/zigma, paths relative to /root/reference):
@@ -267,8 +267,8 @@ typedef struct {
 int zg_block_tail_bwd(const zg_block_tail_bwd_params *p, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
- * bf16 GEMM on tcgen05 tensor cores:  C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]), fp32 accumulate in
- * TMEM, bf16 output.  A, B row-major with leading dims lda/ldb (elements, multiples of 8);
+ * bf16 GEMM on the Hopper tensor cores (wgmma):  C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]), fp32 accumulate in
+ * registers, bf16 output.  A, B row-major with leading dims lda/ldb (elements, multiples of 8);
  * C row-major ldc.  out_rowmap (int32[rows_per_batch] or NULL): output row m of batch
  * m / rows_per_batch is stored at row out_rowmap[m % rows_per_batch] of that batch (scatter of
  * the out_proj result back to raster order, mamba_simple.py:388-394).

@@ -1,10 +1,10 @@
 #!/bin/bash
 # TEST/BENCH INFRASTRUCTURE -- compiles the REFERENCE's own CUDA extensions (vendored mamba_ssm
-# selective_scan + causal_conv1d, unmodified sources where they lie under /root/reference) for sm_100a
+# selective_scan + causal_conv1d, unmodified sources where they lie in the reference checkout, $ZIGMA_REFERENCE_ROOT) for sm_90a
 # into oracle/_ref/{selective_scan_cuda,causal_conv1d_cuda}.so, with the reference's own nvcc flags
 # (dis_mamba/setup.py:137-156, dis_causal_conv1d/setup.py) and only the -gencode swapped: the shipped
-# setup.py files target sm_70/80/90 only (dis_mamba/setup.py:108-114) and do not run on B200.
-# Nothing is copied into the repo; outputs are git-ignored but travel to the GPU box with gpurun.
+# setup.py files target sm_70/80/90 only (dis_mamba/setup.py:108-114) and carry no sm_90a target.
+# Nothing is copied into the repo; the outputs are git-ignored.
 # They are the "reference vendored CUDA path" baseline that bench.py times next to our kernels.
 set -e
 REF=${ZIGMA_REFERENCE_ROOT:-/root/reference}
@@ -23,7 +23,7 @@ PYEOF
 TLIB=$($PY -c "import torch, os; print(os.path.join(os.path.dirname(torch.__file__), 'lib'))")
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 COMMON="-O3 -std=c++17 -Xcompiler -fPIC -DTORCH_API_INCLUDE_EXTENSION_H -D_GLIBCXX_USE_CXX11_ABI=1 $INC"
-NVF="$COMMON -U__CUDA_NO_HALF_OPERATORS__ -U__CUDA_NO_HALF_CONVERSIONS__ -U__CUDA_NO_BFLOAT16_OPERATORS__ -U__CUDA_NO_BFLOAT16_CONVERSIONS__ -U__CUDA_NO_BFLOAT162_OPERATORS__ -U__CUDA_NO_BFLOAT162_CONVERSIONS__ --expt-relaxed-constexpr --expt-extended-lambda --use_fast_math -lineinfo -gencode arch=compute_100a,code=sm_100a -w"
+NVF="$COMMON -U__CUDA_NO_HALF_OPERATORS__ -U__CUDA_NO_HALF_CONVERSIONS__ -U__CUDA_NO_BFLOAT16_OPERATORS__ -U__CUDA_NO_BFLOAT16_CONVERSIONS__ -U__CUDA_NO_BFLOAT162_OPERATORS__ -U__CUDA_NO_BFLOAT162_CONVERSIONS__ --expt-relaxed-constexpr --expt-extended-lambda --use_fast_math -lineinfo -gencode arch=compute_90a,code=sm_90a -w"
 build_ext () {   # name srcdir
     local name=$1 dir=$2; shift 2
     local objs=() pids=()

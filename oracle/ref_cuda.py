@@ -1,6 +1,6 @@
 """BENCH/TEST INFRASTRUCTURE -- the reference's OWN compiled CUDA kernels (oracle/_ref/*.so, built
 from the unmodified sources under /root/reference by oracle/build_ref.sh, gencode swapped to
-sm_100a) behind the restated glue of oracle/zigma_oracle.py: the "reference vendored CUDA path"
+sm_90a) behind the restated glue of oracle/zigma_oracle.py: the "reference vendored CUDA path"
 baseline that BASELINE.md section 5 asks to time on the same box.  Never imported by the product
 package; bench.py uses it only to report the baseline next to our numbers.
 

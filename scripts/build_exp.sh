@@ -5,11 +5,11 @@ set -e
 cd "$(dirname "$0")/.."
 name=$1; extra=${2:--DZG_SCAN_EXP=$1}; tu=${3:-scan_fwd_bf16.cu}
 mkdir -p build/exp/obj$name
-FLAGS="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC $extra"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC $extra"
 for f in zigma_b200/csrc/*.cu; do
   o=build/exp/obj$name/$(basename ${f%.cu}).o
   case $(basename $f) in $tu) nvcc $FLAGS -c $f -o $o & ;; *) cp build/obj/$(basename ${f%.cu}).o $o ;; esac
 done
 wait
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o zigma_b200/lib/libzigma_exp$name.so build/exp/obj$name/*.o -lcudart -lcuda
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o zigma_b200/lib/libzigma_exp$name.so build/exp/obj$name/*.o -lcudart -lcuda
 echo built zigma_b200/lib/libzigma_exp$name.so

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (zg_gemm_bf16_tn) vs the library GEMM at the four projection shapes of BASELINE config 2."""
+"""wgmma GEMM (zg_gemm_bf16_tn) vs the library GEMM at the four projection shapes of BASELINE config 2."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, torch.nn.functional as F
@@ -22,4 +22,4 @@ for name, N, K in (("in_proj", 2560, 640), ("out_proj", 640, 1280), ("x_proj", 7
     t_lib = timeit(lambda: F.linear(x, w))
     fl = 2.0 * M * N * K
     err = (linear_bf16(x, w).float() - F.linear(x, w).float()).abs().max().item()
-    print(f"{name:9s} M={M} N={N} K={K}: tcgen05 {t_ours*1e3:7.1f} us ({fl/t_ours/1e9:7.1f} TFLOP/s)   library {t_lib*1e3:7.1f} us ({fl/t_lib/1e9:7.1f} TFLOP/s)   max|diff| {err:.3e}")
+    print(f"{name:9s} M={M} N={N} K={K}: wgmma {t_ours*1e3:7.1f} us ({fl/t_ours/1e9:7.1f} TFLOP/s)   library {t_lib*1e3:7.1f} us ({fl/t_lib/1e9:7.1f} TFLOP/s)   max|diff| {err:.3e}")

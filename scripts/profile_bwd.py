@@ -1,4 +1,4 @@
-"""One launch of every TRAINING kernel at the BASELINE config-2 layer shape (token-major, bf16) for ncu."""
+"""One launch of every TRAINING kernel at the BASELINE config-2 layer shape (token-major, bf16), to run under a profiler."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

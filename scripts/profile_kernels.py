@@ -1,4 +1,4 @@
-"""One launch of every hot-path kernel at the BASELINE config-2 layer shape, for `ncu --set full` captures."""
+"""One launch of every hot-path kernel at the BASELINE config-2 layer shape, to run under a profiler."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -26,7 +26,7 @@ x = torch.randn(bs, L, D, device=dev, generator=g).to(dt); mix = torch.randn(bs,
 mods = torch.randn(bs, 3 * D, device=dev, generator=g).to(dt); res = torch.randn(bs, L, D, device=dev, generator=g); nw = torch.ones(D, device=dev).to(dt)
 Win = (torch.randn(2 * E, D, device=dev, generator=g) / D ** 0.5).to(dt)
 Wout = (torch.randn(D, E, device=dev, generator=g) / E ** 0.5).to(dt)
-for it in range(2):     # first pass warms up (attributes, caches); profile the second (ncu -s)
+for it in range(2):     # first pass warms up (attributes, caches); profile the second
     torch.cuda.synchronize()
     if it == 1: torch.cuda.profiler.start()
     _scan_fwd(xc.transpose(1, 2), dl.transpose(1, 2), A, Bv, Cv, Dp, xz[:, :, E:].transpose(1, 2), bias, True, z_rowmap=perm, want_last_state=False)

@@ -85,11 +85,13 @@ def test_ops_fail_loudly_without_cuda():
 
 def test_scan_kernel_choice_shape_rule():
     """zg_scan_kernel_choice (the pure part of scan_auto_choice, scan_fwd.cuh): which hot-path forward-scan kernel a call gets on a
-    148-SM B200.  The BASELINE workloads per GPU: config 2 -> CTAs of 8 wide + 2 narrow warps (9 units on every sub-partition),
-    FacesHQ-1024 and both video layer shapes -> 32-channel warps, small batches and the training forward -> the CTA-wide kernel."""
+    132-SM H100.  The BASELINE workloads per GPU: config 2 (more than 36 units per SM: several waves), FacesHQ-1024 and both video
+    layer shapes -> 32-channel warps, small batches and the training forward -> the CTA-wide kernel; one-wave batches in between
+    -> mixed CTAs of wide + narrow warps."""
     from zigma_b200 import _lib
     ch = _lib.scan_kernel_choice
-    assert ch(64, 1280) == (5, 8, 2)                       # zigzag8_b1 / sweep2_b1, bs 64
+    assert ch(64, 1280) == (3, 0, 0)                       # zigzag8_b1 / sweep2_b1, bs 64
+    assert ch(64, 1280, sms=148) == (5, 8, 2)              # (the same call on a device of 148 SMs: 8 wide + 2 narrow warps)
     assert ch(32, 1536) == (3, 0, 0)                       # faceshq1024, bs 32
     assert ch(16 * 16, 1536) == (3, 0, 0)                  # ucf101_sst spatial layers: 256 sequences
     assert ch(16 * 256, 1536) == (3, 0, 0)                 # ucf101_sst temporal layers: 4096 sequences
@@ -102,5 +104,5 @@ def test_scan_kernel_choice_shape_rule():
         assert mode in (0, 3, 5)
         if mode == 5:
             assert nd in (4, 8) and ns % 2 == 0 and 0 <= ns and nd + ns <= 10
-            units_per_sm = -(-bs * 80 // 148)
+            units_per_sm = -(-bs * 80 // 132)
             assert 2 * (2 * nd + ns) >= units_per_sm       # two CTAs per SM hold the SM's share: one wave

@@ -1,4 +1,4 @@
-"""GPU (B200): backward kernels (selective_scan_cuda.bwd / causal_conv1d_bwd / layer-norm bwd
+"""GPU (H100): backward kernels (selective_scan_cuda.bwd / causal_conv1d_bwd / layer-norm bwd
 replacements) against the reference's autograd gradients (golden) and the differentiable oracle."""
 import numpy as np
 import pytest

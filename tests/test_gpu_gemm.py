@@ -1,4 +1,4 @@
-"""GPU (B200): the hand-written tcgen05 GEMM (zg_gemm_bf16_tn) against torch.matmul in fp32 on the same
+"""GPU (H100): the hand-written wgmma GEMM (zg_gemm_bf16_tn) against torch.matmul in fp32 on the same
 bf16 operands, at the four projection shapes of the hot path and at ragged shapes."""
 import pytest
 import torch
@@ -17,6 +17,7 @@ SHAPES = [
     (1000, 200, 136),             # everything ragged
     (128, 64, 64), (1, 8, 8), (129, 257, 72),
     (4096, 80, 1536), (4096, 768, 1536),   # x_proj / out_proj of the D = 768 models (80-wide tile; 3 x 256)
+    (300, 5184, 72),              # 256-wide tiles whose last column tile holds 64 valid columns: its other chunks store nothing
     (300, 160, 64), (257, 150, 200), (520, 330, 96),   # 160-wide tiles: exact, ragged in N (tail columns by direct stores), two tiles + ragged
 ]
 
@@ -61,7 +62,7 @@ def test_gemm_row_scatter_and_views():
 
 
 def test_engine_with_tcgen05_gemms(monkeypatch):
-    """Whole bf16 model with the projections routed through zg_gemm_bf16_tn == library-GEMM engine."""
+    """Whole bf16 model with the projections routed through zg_gemm_bf16_tn (ZIGMA_TCGEN05=1, the historical name of the switch) == library-GEMM engine."""
     from oracle import synth
     from oracle.gen_golden import model_io
     from util import model_case
@@ -75,5 +76,5 @@ def test_engine_with_tcgen05_gemms(monkeypatch):
         x, tt, _ = model_io(cfg, 2)
         with torch.no_grad():
             outs[flag] = m(x.to(DEV).bfloat16(), tt.to(DEV).bfloat16()).float()
-    check_close(outs["1"], outs["0"], "engine tcgen05 vs library GEMMs", rtol=3e-2, atol=3e-2, scale_atol=False, max_strict_viol=1.0)
-    check_close(outs["1"], g["out"], "engine tcgen05 vs reference bf16", rtol=5e-2, atol=5e-2, scale_atol=False, max_strict_viol=1.0)
+    check_close(outs["1"], outs["0"], "engine wgmma vs library GEMMs", rtol=3e-2, atol=3e-2, scale_atol=False, max_strict_viol=1.0)
+    check_close(outs["1"], g["out"], "engine wgmma vs reference bf16", rtol=5e-2, atol=5e-2, scale_atol=False, max_strict_viol=1.0)

@@ -1,4 +1,4 @@
-"""GPU (B200): ZigMa.forward / mamba_inner_fn end to end against the golden vectors produced by the
+"""GPU (H100): ZigMa.forward / mamba_inner_fn end to end against the golden vectors produced by the
 unmodified reference, through both execution paths (engine fast path and autograd path)."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU (B200): parity of every op of the C-ABI against the oracle / the reference's golden vectors.
+"""GPU (H100): parity of every op of the C-ABI against the oracle / the reference's golden vectors.
 All calls go through the host mirror of the reference interface -> ctypes -> libzigma_b200.so."""
 import numpy as np
 import pytest
@@ -335,9 +335,11 @@ def test_selective_scan_properties_full_size():
     from zigma_b200 import _lib
     out = run(u, delta, z, Bv, Cv)
     assert out.shape == (Bt, E, L) and torch.isfinite(out.float()).all()
-    auto = "ZG_SCAN_WP" not in os.environ and torch.cuda.get_device_properties(0).multi_processor_count == 148
-    if auto:    # scan_auto_choice: 5120 units on 148 SMs -> CTAs of 8 wide + 2 narrow warps
-        assert "scan_fwd_wph_kernel" in _lib.last_scan_kernel(), _lib.last_scan_kernel()
+    auto = "ZG_SCAN_WP" not in os.environ
+    if auto:    # scan_auto_choice: 5120 units on this device's SMs (132 SMs -> 32-channel warps)
+        mode = _lib.scan_kernel_choice(Bt, E, sms=torch.cuda.get_device_properties(0).multi_processor_count)[0]
+        want = {0: "scan_fwd_tma_kernel", 3: "scan_fwd_wp2_kernel", 5: "scan_fwd_wph_kernel"}[mode]
+        assert mode in (3, 5) and want in _lib.last_scan_kernel(), _lib.last_scan_kernel()
     # causality
     u2, d2, z2, x2 = u.clone(), delta.clone(), z.clone(), xbc.clone()
     u2[:, L // 2:] = 0; d2[:, L // 2:] = 0; z2[:, L // 2:] = 1; x2[:, L // 2:] = 0

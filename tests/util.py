@@ -33,7 +33,7 @@ def check_close(actual, expected, what, rtol=RTOL, atol=ATOL, scale_atol=True, m
       scales with the output range;
     * strict bound: the fraction of elements violating the UNSCALED north-star tolerance
       (rtol 1e-3, atol 1e-5) must stay below max_strict_viol (default 1e-4; measured on BASELINE
-      config 1: 7.6e-7 between the two CPU fp32 implementations, 3.2e-5 for the sm_100a kernel
+      config 1: 7.6e-7 between the two CPU fp32 implementations, 3.2e-5 for the sm_90a kernel
       whose exp2/log2/rcp are MUFU approximations of ~2^-22 relative error).
     """
     a = torch.as_tensor(actual).detach().float().cpu()
@@ -54,16 +54,15 @@ def check_close(actual, expected, what, rtol=RTOL, atol=ATOL, scale_atol=True, m
 
 
 def _log_parity(what, max_diff, max_ref, strict, hard_viol, numel, rtol, atol, max_strict_viol):
-    """Appends the achieved error of every check to gpurun_out/parity_log.jsonl (GPU runs only), so the numbers behind
-    "N passed" survive the run; scripts/parity_summary.py condenses the file into profiles/."""
-    if not torch.cuda.is_available():
+    """With ZIGMA_PARITY_LOG=<file> in the environment, appends the achieved error of every check to that JSON-lines file, so
+    the numbers behind "N passed" survive the run.  Nothing is written otherwise (the source tree may be read-only)."""
+    path = os.environ.get("ZIGMA_PARITY_LOG")
+    if not path:
         return
     try:
-        d = os.path.join(ROOT, "gpurun_out")
-        os.makedirs(d, exist_ok=True)
         rec = dict(test=os.environ.get("PYTEST_CURRENT_TEST", "").split(" ")[0], what=what, max_diff=max_diff, max_ref=max_ref,
                    strict_viol_frac=strict, hard_viol=hard_viol, numel=numel, rtol=rtol, atol=atol, max_strict_viol=max_strict_viol)
-        with open(os.path.join(d, "parity_log.jsonl"), "a") as f:
+        with open(path, "a") as f:
             f.write(json.dumps(rec) + "\n")
     except OSError:
         pass

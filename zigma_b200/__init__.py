@@ -1,10 +1,10 @@
-"""zigma_b200 -- B200-native (sm_100a) implementation of the ZigMa denoiser hot path.
+"""zigma_b200 -- H100-native (sm_90a) implementation of the ZigMa denoiser hot path.
 
 Public surface mirrors the reference (CompVis/zigma):
     ZigMa, Mamba, selective_scan_fn, mamba_inner_fn, mamba_inner_fn_no_out_proj, bimamba_inner_fn,
     causal_conv1d_fn, rms_norm_fn, layer_norm_fn, RMSNorm, zigzag_path, hilbert_path,
     reverse_permut_np, create_transport, Sampler
-plus what sits around the path on a B200 node: train_step / FlatParams / GradSync / FusedAdamWEMA (zigma_b200.train),
+plus what sits around the path on an H100 node: train_step / FlatParams / GradSync / FusedAdamWEMA (zigma_b200.train),
 load_reference_checkpoint / save_reference_checkpoint (zigma_b200.checkpoint), decode_latents / to_uint8_pixels (zigma_b200.handoff:
 the VAE-decode hand-off after sampling).
 All arithmetic on the path runs in libzigma_b200.so (include/zigma_b200.h); there is no CPU fallback.

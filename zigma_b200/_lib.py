@@ -1,4 +1,4 @@
-"""ctypes binding of the C-ABI in include/zigma_b200.h (libzigma_b200.so, sm_100a).
+"""ctypes binding of the C-ABI in include/zigma_b200.h (libzigma_b200.so, sm_90a).
 
 There is NO fallback: if the shared library is missing or a call fails, a RuntimeError is raised
 (the reference raises RuntimeError from TORCH_CHECK the same way, selective_scan.cpp:226-336).
@@ -105,7 +105,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"zigma_b200: native library {LIB_PATH} not found -- build it with "
-                f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). There is no CPU/PyTorch fallback.")
+                f"`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). There is no CPU/PyTorch fallback.")
         l = C.CDLL(LIB_PATH)
         l.zg_last_error.restype = C.c_char_p
         l.zg_launch_count.restype = C.c_uint64
@@ -124,7 +124,7 @@ def launch_count():
     return int(lib().zg_launch_count())
 
 
-def scan_kernel_choice(batch, dim, sms=148, training_forward=False):
+def scan_kernel_choice(batch, dim, sms=132, training_forward=False):
     """(mode, wide warps, narrow warps) the shape rule picks for a hot-path forward-scan call (zg_scan_kernel_choice; host arithmetic)."""
     nd, ns = C.c_int32(0), C.c_int32(0)
     mode = lib().zg_scan_kernel_choice(int(batch) * (int(dim) // 16), int(sms), int(bool(training_forward)), C.byref(nd), C.byref(ns))
@@ -159,4 +159,4 @@ def ptr(t):
 def require_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("zigma_b200: expected CUDA tensors (the kernels are sm_100a only; there is no CPU path)")
+            raise RuntimeError("zigma_b200: expected CUDA tensors (the kernels are sm_90a only; there is no CPU path)")

@@ -8,7 +8,7 @@
 Forward: ``zg_block_tail_fwd`` (one pass, the reference's bf16 rounding points replicated); backward:
 ``zg_block_tail_bwd`` (one pass: RMSNorm backward, d_mix scattered back to scan order, dgate / dshift / dscale /
 d_norm_w column sums in registers).  The unfused graph costs ~12 elementwise / reduction kernels per block and
-direction (14 % of a training step on B200, DESIGN.md section 5).
+direction (DESIGN.md section 4.4).
 """
 import torch
 

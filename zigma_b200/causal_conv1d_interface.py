@@ -1,5 +1,5 @@
 """Host-side mirror of ``dis_causal_conv1d/causal_conv1d/causal_conv1d_interface.py`` (reference)
-over the sm_100a kernels: ``causal_conv1d_fn`` (:37-46) with its autograd Function (:10-34).
+over the sm_90a kernels: ``causal_conv1d_fn`` (:37-46) with its autograd Function (:10-34).
 ``causal_conv1d_update`` (single-token decode, :68-80) is out of scope: diffusion sampling never
 decodes autoregressively (SURVEY.md section 2 #4)."""
 import torch

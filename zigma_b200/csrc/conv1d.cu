@@ -1,4 +1,4 @@
-// Depthwise causal conv1d (+bias, +SiLU) forward / backward for sm_100a.
+// Depthwise causal conv1d (+bias, +SiLU) forward / backward for sm_90a.
 //
 // Replaces causal_conv1d_fwd_kernel / causal_conv1d_channellast_fwd_kernel and their backward
 // (dis_causal_conv1d/csrc/causal_conv1d_fwd.cu:39-158,193-330, causal_conv1d_bwd.cu:46-505).
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(128, 5) conv_fwd_dimc_kernel(const zg_conv_par
     }
 }
 
-// forward, token-major fast path: 16-bit I/O, 4 channels per thread as two fp32x2 pairs (FFMA2 taps), seqlen a
+// forward, token-major fast path: 16-bit I/O, 4 channels per thread as two fp32 pairs (zg_f2 taps), seqlen a
 // multiple of CONV_LCH, everything 8-byte aligned.  ~10 issued instructions per output element instead of
 // the generic kernel's 28 (ncu round 1: the generic kernel was instruction-issue bound at 52 % issue
 // utilisation, 130 us for 335 MB).
@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(128, ZG_CONV_MINB) conv_fwd_tok4_kernel(const 
 // rows in flight in a per-lane shared-memory ring (3 batches x 8 rows x 16 B) while it computes the third: 128 KB in flight per SM with
 // 16 resident warps, no registers spent on data in flight.  Every lane reads back exactly the 16 bytes it copied itself, so its own
 // cp.async.wait_group is the only synchronisation (no barrier, no __syncwarp).  Same arithmetic and rounding as conv_fwd_tok4_kernel
-// (packed FFMA2 taps in the same order, the same SiLU): bit-identical results.
+// (zg_f2 taps in the same order, the same SiLU): bit-identical results.
 constexpr int CS_ROWS = 8, CS_STAGES = 3, CS_WARPS = 4, CS_CH = 256;          // rows per batch, ring depth, warps per CTA, channels per warp
 constexpr int CS_WARP_BYTES = CS_STAGES * CS_ROWS * CS_CH * 2;                // 12 KB
 template <typename T, int LCH>
@@ -690,7 +690,7 @@ __global__ void __launch_bounds__(128, (DV <= 2) ? 6 : 4) conv_bwd_tok_kernel(co
 // as conv_bwd_tok_kernel but branch-free -- chunks are whole, the three halo positions either all exist (another chunk
 // follows) or none does, so the per-position bounds tests, the divergent branches and most of the address arithmetic of
 // the generic kernel go away (ncu round 1: 66 issued instructions per channel-position there, ~25 needed), rows are
-// fetched CONV_B4_RB at a time one batch ahead, taps run as packed FFMA2 on channel pairs.
+// fetched CONV_B4_RB at a time one batch ahead, taps run as zg_f2 FMAs on channel pairs.
 constexpr int CONV_B4_LCH = 32;
 constexpr int CONV_B4_RB = 4;
 

@@ -1,4 +1,4 @@
-// Fused residual-add + RMSNorm/LayerNorm (forward, backward) and the fused ZigMa block tail, sm_100a.
+// Fused residual-add + RMSNorm/LayerNorm (forward, backward) and the fused ZigMa block tail, sm_90a.
 //
 // Replaces the Triton kernels _layer_norm_fwd_1pass_kernel / _layer_norm_bwd_kernel
 // (dis_mamba/mamba_ssm/ops/triton/layernorm.py:64-120,195-290) and, for the inference fast path,
@@ -426,7 +426,7 @@ __global__ void __launch_bounds__(128, (MAXQ <= 6) ? 6 : 1) block_tail_kernel(co
 #endif
 // Round 2: FOUR warps per row (one 128-thread CTA = one token row).  The one-warp-per-row kernel above keeps a whole row in the
 // registers of 32 lanes (67 registers at D = 640 -> 7 CTAs = 28 warps per SM, 42 % occupancy) and ncu shows it purely
-// latency-bound: long_scoreboard 12.9 warps per issue, issue 36 %, 4.5 TB/s (profiles/r02_tail_conv_ncu.txt).  Spreading the row
+// latency-bound: long_scoreboard 12.9 warps per issue, issue 36 %.  Spreading the row
 // over 128 lanes leaves 1-2 quads per lane (about half the registers, twice the resident warps) at the price of one
 // shared-memory reduction per statistic.  Same arithmetic and rounding points.  Measured at config 2 (672 MB per call):
 // 149.7 us (one warp per row) -> 136.5 us (this kernel, 40 registers, 12 CTAs / SM) -> 121.1 us = 5.54 TB/s = 0.84 of the measured
@@ -782,7 +782,7 @@ template <typename T> static int norm_fwd_t(const zg_norm_params &p, cudaStream_
 }
 template <typename T, typename R> static int norm_bwd_tr(const zg_norm_bwd_params &p, cudaStream_t s) {
     const int64_t want = ((int64_t)p.nrows * 32 + 127) / 128;
-    const unsigned grid = (unsigned)(want < 148 * 4 ? want : 148 * 4);
+    const unsigned grid = (unsigned)(want < 132 * 4 ? want : 132 * 4);
     const uintptr_t al = reinterpret_cast<uintptr_t>(p.dy) | reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(p.dresidual) |
                          reinterpret_cast<uintptr_t>(p.dx) | reinterpret_cast<uintptr_t>(p.dresidual_in);
     const int64_t so = p.dy_rs | p.x_rs | p.dx_rs | (p.dresidual ? p.dres_rs : 0) | (p.dresidual_in ? p.dresin_rs : 0);

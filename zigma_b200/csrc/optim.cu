@@ -1,4 +1,4 @@
-// Fused AdamW + EMA step over one FLAT fp32 parameter buffer (sm_100a).
+// Fused AdamW + EMA step over one FLAT fp32 parameter buffer (sm_90a).
 //
 // Replaces, for the training loop around the denoiser (train_acc.py:442-448 of the reference):
 //   opt.step()                      torch.optim.AdamW (lr, weight_decay; betas (0.9, 0.999), eps 1e-8 defaults, :213-215)
@@ -64,7 +64,7 @@ extern "C" int zg_adamw_ema_step(const zg_adamw_params *pp, void *stream) {
     if (p.n == 0) return 0;
     const int64_t n4 = (p.n + 3) >> 2;
     int64_t blocks = (n4 + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;          // grid-stride: 8 CTAs of 256 threads per SM
+    if (blocks > 132 * 8) blocks = 132 * 8;          // grid-stride: 8 CTAs of 256 threads per SM
     zg::adamw_ema_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(p);
     zg_count_launch();
     return zg_check_launch("adamw_ema_step");

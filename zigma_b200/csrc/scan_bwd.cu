@@ -1,4 +1,4 @@
-// Selective-scan (S6) backward for sm_100a -- same mapping as the forward (scan_fwd.cuh): a thread
+// Selective-scan (S6) backward for sm_90a -- same mapping as the forward (scan_fwd.cuh): a thread
 // owns one channel, keeps dh / dA partial sums in registers and walks L in reverse, one 8-step chunk
 // at a time (generic fallback: any dstate <= 64, constant (dim, dstate) B / C; the dstate == 16 input-dependent case runs
 // scan_bwd_q4.cuh).  Replaces

@@ -1,7 +1,7 @@
-// Selective-scan backward, dstate == 16 specialisation for sm_100a: FOUR threads per channel, four
+// Selective-scan backward, dstate == 16 specialisation for sm_90a: FOUR threads per channel, four
 // states each ("quad" = lanes 4j..4j+3 of a warp), 64 channels x one batch row per 256-thread CTA.
 // Same math as the generic kernel in scan_bwd.cu (reference: selective_scan_bwd_kernel.cuh:186-213,
-// 252-296,439-452); what changes is the mapping, chosen for occupancy and memory behaviour on B200:
+// 252-296,439-452); what changes is the mapping, chosen for occupancy and memory behaviour:
 //
 //   * parked states (h_{l-1} of the 8 steps of a chunk, recomputed from the forward's checkpoint)
 //     cost 64 B per (channel, step) whatever the thread mapping -- with 4 threads per channel that is
@@ -18,7 +18,7 @@
 //   * dB / dC (sums over the channels that share a group): 7-shuffle transpose-reduce over the 8
 //     channels of a warp, cross-warp sum through shared memory, then one fp32 atomic per
 //     (CTA, state, step) with 8 consecutive steps per 32-byte sector;
-//   * packed FFMA2 math on state pairs, as in the forward;
+//   * zg_f2 pair math on state pairs, as in the forward;
 //   * z_rowmap (the forward's fused permutation of the gate) redirects the z reads and the dz writes.
 #pragma once
 #include "zg_common.cuh"

@@ -1,10 +1,10 @@
-// Selective-scan (S6) forward for sm_100a -- sequential-in-L, parallel over (batch, channel, state).
+// Selective-scan (S6) forward for sm_90a -- sequential-in-L, parallel over (batch, channel, state).
 //
 // Replaces selective_scan_fwd_kernel (dis_mamba/csrc/selective_scan/selective_scan_fwd_kernel.cuh:67-303).
 // The reference maps one CTA to one (batch, channel) row and runs a CUB block scan over L for each
 // of the N states in turn (17.4 issued SASS instructions per (b,d,l,n) update, 3 BAR.SYNC per state
 // iteration, SURVEY.md section 8a).  At the batch sizes of the sampling path there are B*E >= 80k
-// independent recurrences -- more than enough to fill 148 SMs without parallelising over L -- so here
+// independent recurrences -- more than enough to fill 132 SMs without parallelising over L -- so here
 // every THREAD owns one channel, keeps its N states in registers and walks L sequentially:
 // 1 FMUL + 1 MUFU.EX2 + 1 FMUL + 2 FFMA per state update, no block-wide scan, no shuffles.
 // The (u, delta, z) tiles and the B/C rows of the next steps are staged into shared memory by a
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(SCAN_CH, (NS <= 16 && !CONSTBC) ? SCAN_MIN_CTA
 
     // ---- per-thread constants and state --------------------------------------------------------
     // states live in registers as fp32x2 PAIRS (n, n+1): every FMA-pipe instruction of the inner loop
-    // is a packed FFMA2/FMUL2, halving the issue slots of the recurrence.
+    // is one zg_f2 pair operation (two scalar fp32 instructions on sm_90a, which has no packed form).
     zg_f2 Al2p[NP], h2[NP];
     float Bc[CONSTBC ? NS : 1], Cc[CONSTBC ? NS : 1];
 #pragma unroll
@@ -436,7 +436,7 @@ int launch_scan_fwd(const zg_scan_params &p, cudaStream_t stream) {
     return zg_check_launch("scan_fwd");
 }
 
-// How many state pairs use the polynomial exp2 (tuning knob; default chosen from the B200 measurements
+// How many state pairs use the polynomial exp2 (tuning knob; default carried over from measurements on another GPU; not re-tuned on H100
 // in DESIGN.md).  ZG_SCAN_NPOLY in the environment overrides it (read once).
 inline int scan_npoly_setting() {
     static int v = -1;

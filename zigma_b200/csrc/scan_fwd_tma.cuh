@@ -6,7 +6,7 @@
 // (delta bias + softplus), :216-261 (the recurrence h = exp(delta A) h + delta u B, y = C h), :280-298 (D skip, SiLU(z)
 // gate) and, for the fused prologue, selective_scan_interface.py:323 (delta = dt_proj.weight @ x_dbl[:, :R].t()).
 //
-// Why a rewrite (round-1 ncu of scan_fwd_tpc2_kernel, profiles/r01_kernels_ncu.txt): 141 issued instructions per
+// Why a rewrite (profile of scan_fwd_tpc2_kernel on the GPU it was first tuned on): 141 issued instructions per
 // (b, e, l) against 48 of state arithmetic and 20 MUFU; issue 59 %, XU 67 %.  The per-step scalar work (softplus, SiLU,
 // bf16 unpacking, two SHFLs, per-thread LDGSTS address arithmetic, 2-byte stores) sat inside the recurrence loop of every
 // thread, and three block barriers per 16 steps kept the four warps of a CTA in lock step.  Here:
@@ -29,7 +29,7 @@
 //              the CTA's dt_proj rows (kept in shared memory), rounded to the I/O dtype like the reference's GEMM output:
 //              the (batch, dim, seqlen) delta tensor never exists in HBM and the dt_proj GEMM launch disappears.
 //   main       two threads per channel, 8 states (4 fp32x2 pairs) each: per step one LDS.64 (delta', delta' u), four
-//              LDS.128 (B, C), 4 x {FMUL2, 2 MUFU.EX2 | polynomial, FMUL2, FFMA2, FFMA2}, one FADD, one STS (the partial
+//              LDS.128 (B, C), 4 x {pair multiply, 2 MUFU.EX2 | polynomial, pair multiply, 2 pair FMAs}, one FADD, one STS (the partial
 //              y overwrites the (delta', delta' u) slot it came from).
 //   post       y = y_lo + y_hi + D u, SiLU(z) gate, bf16x2 pack, 4-byte stores.
 #pragma once
@@ -198,7 +198,7 @@ template <typename T> __device__ __forceinline__ void pt_mma_k8(float &d0, float
 // ddu_c: this channel's (delta', delta' u) pairs, one per step.  ypart: where this thread's partial y of step t goes (+ t * ypitch):
 // with two threads per channel the two halves overwrite the pair they were computed from, else a separate tile.
 // Software-pipelined by hand (ZG_SCAN_SWP, default on): ptxas emits the unrolled steps strictly one after the other
-// (LDS -> FMUL2 -> 8 MUFU -> FFMA2 chain -> STS, ~140 cycles of dependent latency per step and warp), so the decay factors
+// (LDS -> multiplies -> 8 MUFU -> FMA chain -> STS, ~140 cycles of dependent latency per step and warp), so the decay factors
 // exp2(delta' A) of step t + 1 -- which depend on nothing but (delta', A) -- are issued BEFORE the FMA part of step t.
 template <int NP, int TPC, int PITCH = PT_F32ROW>
 __device__ __forceinline__ void pt_main_stage(const unsigned char *__restrict__ ddu_c, const float *__restrict__ bcf_p, unsigned char *__restrict__ ypart, int ypitch,
@@ -668,7 +668,7 @@ template <typename T> inline int wp_dispatch(const zg_scan_params &p, cudaStream
 }
 
 // Which hot-path kernel runs a call (ZG_SCAN_WP unset).  All of them compute the same bits; what differs is how the work
-// quantises over the 4 x SMs sub-partitions and how busy each keeps its MUFU pipe (measured on B200, DESIGN.md section 4.1):
+// quantises over the 4 x SMs sub-partitions and how busy each keeps its MUFU pipe (thresholds carried over from a 148-SM GPU, expressed per SM; not re-tuned on H100):
 // the 32-channel warps of scan_fwd_wp2 reach 85 % of the pipe against 76-79 % for 16-channel warps, but their unit of work is twice
 // as large.  In 16-channel units, with U of them and S SMs, the fullest sub-partition carries
 //     CTA-wide kernel (4 warps, one per sub-partition)      ceil(ceil(U / 4) / S)
@@ -683,7 +683,7 @@ inline ScanChoice scan_auto_choice(const zg_scan_params &p) {
     int dev = 0;
     cudaGetDevice(&dev);
     if (!sms_dev[dev & 63]) cudaDeviceGetAttribute(&sms_dev[dev & 63], cudaDevAttrMultiProcessorCount, dev);
-    return scan_choice_for((long long)(p.dim / 16) * p.batch, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 148, p.ckpt != nullptr);
+    return scan_choice_for((long long)(p.dim / 16) * p.batch, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 132, p.ckpt != nullptr);
 }
 
 // host-side eligibility test + launch; returns -1 when the call does not fit the specialisation (never for a fused request:

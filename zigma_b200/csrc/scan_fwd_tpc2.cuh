@@ -5,12 +5,12 @@
 // work (softplus of one step, SiLU gate + store of one step, exchanged with one SHFL each way).
 //
 // Why: with one thread per channel the kernel needs 96 registers per thread and the grid (B*E/32 = 2560 warps
-// at BASELINE config 2) only supplies 4.3 warps per SM sub-partition; ncu (profiles/r01_scan_fwd_v2.txt) shows
+// at BASELINE config 2) only supplies 4.3 warps per SM sub-partition; a profile of it showed
 // the scheduler with ~1.1 eligible warps per cycle and `wait` (fixed-latency dependency) as the top stall.
 // Splitting the states halves the live registers (<= 56) and doubles the resident warps (8.6 per SMSP) for the
 // same total instruction and MUFU count, so the MUFU pipe -- the real bound of this kernel -- stays fed.
 //
-// Tried and rejected (round 1, gpurun call 35): a warp-autonomous variant (every warp stages / converts / consumes its own
+// Tried and rejected (an earlier experiment): a warp-autonomous variant (every warp stages / converts / consumes its own
 // 8-step tiles, __syncwarp instead of the three block barriers per 16 steps) -- bit-identical results, 0.638 ms instead of
 // 0.557 ms: the extra per-warp staging work and the 4x B/C traffic cost more than the barriers do.
 #pragma once

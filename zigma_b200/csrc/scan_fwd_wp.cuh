@@ -1,7 +1,7 @@
 // Selective-scan forward, warp-private pipeline (round 2, second half): the arithmetic of scan_fwd_tma_kernel with every
 // warp running its own staging ring -- no block barrier anywhere in the stage loop.
 //
-// Why (ncu of scan_fwd_tma_kernel, profiles/r02_scan_fwd_ncu.txt): the kernel is bounded by the MUFU pipe (16 exp2 + 4 per
+// Why (profile of scan_fwd_tma_kernel on the GPU it was first tuned on): the kernel is bounded by the MUFU pipe (16 exp2 + 4 per
 // (b, e, l)), yet that pipe is busy only 76 % of the time.  10 % of the stall samples sit on the instruction after the two
 // BAR.SYNC of a stage, and only 6.2 of the 8.65 resident warps per sub-partition are alive on average: the four warps of a CTA
 // live on four different sub-partitions, each of which schedules oldest-first, so a warp that is favoured on its own
@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(32 * WP_MAX_WARPS, 2) scan_fwd_wp_kernel(const
 }
 
 // CTA shape.  The warps exchange nothing, so the CTA size is free; what it decides is how the SM's warp schedulers treat the
-// warps.  ncu of 4- / 5-warp CTAs (gpurun_out/r02b_scan_wp1_np0): only 6.1 of the 8.75 resident warps per sub-partition are alive
+// warps.  ncu of 4- / 5-warp CTAs: only 6.1 of the 8.75 resident warps per sub-partition are alive
 // on average although every warp has the same work -- the schedulers favour the oldest warps, those finish at ~40 % of the
 // kernel time, and the youngest ones run the tail with too few peers to keep the MUFU pipe busy (74 % over the whole kernel).
 // When the whole problem fits one wave, the warps of an SM are therefore packed into ONE or TWO large CTAs whose warps meet at a
@@ -291,7 +291,7 @@ template <typename T, bool CKPT, bool PLAIN, bool TMA, int NPOLY = 0> int wp_lau
         attr_dev[dev & 63] = true;
     }
     const long long units = (long long)(p.dim / WP_CH) * p.batch;
-    const WpShape sh = wp_pick_shape(units, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 148);
+    const WpShape sh = wp_pick_shape(units, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 132);
     const int w = sh.warps;
     const long long nblk = (units + w - 1) / w;
     kern<<<(unsigned)nblk, 32 * w, w * LY::WARP_BYTES, stream>>>(p, maps, sh.sync_every);

@@ -1,6 +1,6 @@
 // Selective-scan forward, warp-private pipeline with TWO channels per lane (32 channels x 16 states per warp).
 //
-// Why: ncu of both hot-path kernels (gpurun_out/r02b_scan_wp*.ncu-rep) shows a second resource next to the MUFU pipe: the
+// Why: ncu of both hot-path kernels shows a second resource next to the MUFU pipe: the
 // shared-memory data pipe of the SM runs 55 % (CTA-wide kernel) / 72 % (warp-private, one channel per lane) of its wavefront
 // peak, three quarters of it the B / C rows of the recurrence: every lane fetches its eight B and eight C values per step
 // (4 LDS.128 = 2048 lane-bytes = 8 wavefronts per warp-step, broadcast or not), and those loads share the sub-partition's MIO
@@ -323,7 +323,7 @@ template <typename T, bool CKPT, bool PLAIN, bool TMA> int wp2_launch(const zg_s
         attr_dev[dev & 63] = true;
     }
     const long long units = (long long)(p.dim / WP2_CH) * p.batch;
-    const int w = wp2_pick_warps(units, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 148);
+    const int w = wp2_pick_warps(units, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 132);
     const long long nblk = (units + w - 1) / w;
     kern<<<(unsigned)nblk, 32 * w, w * LY::WARP_BYTES, stream>>>(p, maps);
     zg_count_launch();

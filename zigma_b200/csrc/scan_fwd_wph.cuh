@@ -2,7 +2,7 @@
 // `ns` warps own 16 (one per lane, wp_body).
 //
 // Why: the two-channels-per-lane warp keeps the MUFU pipe of its sub-partition 85 % busy (against 76-79 % of the one-channel
-// kernels: gpurun_out/r02d_scan_wp3.ncu-rep), but its unit of work is twice as large, and at BASELINE config 2 the work does not
+// kernels), but its unit of work is twice as large, and at BASELINE config 2 the work does not
 // divide: 81 920 channels / 592 sub-partitions = 8.65 units of 16 channels.  Whole 32-channel warps put 5 of them = 10 units on
 // the fullest sub-partition (smsp__inst_executed max / avg = 1.16) and the kernel takes as long as before.  Four 32-channel warps
 // plus one 16-channel warp per sub-partition are 9 units: the quantisation of the one-channel kernels with (mostly) the
@@ -69,7 +69,7 @@ template <typename T, bool CKPT, bool PLAIN> int wph_launch(const zg_scan_params
 }
 
 // mode 5.  nd wide + ns narrow warps per CTA: the caller's choice (scan_auto_choice), else ZG_SCAN_WPH_ND / ZG_SCAN_WPH_NS
-// (default 8 + 2: config 2 on 148 SMs).
+// (default 8 + 2).
 template <typename T> int wph_launch_variant(const zg_scan_params &p, cudaStream_t stream, int nd, int ns) {
     if (nd <= 0) { nd = pt_env_int("ZG_SCAN_WPH_ND", 8); ns = pt_env_int("ZG_SCAN_WPH_NS", 2); }
     if (nd < 0 || ns < 0 || nd + ns < 1 || nd + ns > WPH_MAX_WARPS || (ns & 1)) { nd = 8; ns = 2; }     // (an even number of narrow warps: a CTA starts at an even unit)

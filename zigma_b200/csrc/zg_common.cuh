@@ -1,4 +1,4 @@
-// Shared device/host helpers for the zigma_b200 kernels (sm_100a only).
+// Shared device/host helpers for the zigma_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -68,14 +68,13 @@ __device__ __forceinline__ float zg_softplus20(float x) {
 __device__ __forceinline__ float zg_sigmoid(float x) { return zg_rcp(1.f + zg_ex2(-x * ZG_LOG2E)); }
 __device__ __forceinline__ float zg_silu(float x) { return x * zg_sigmoid(x); }
 
-// ---- packed fp32x2 arithmetic (FFMA2 / FMUL2 / FADD2 on sm_100a: one issue slot, two results) ----
-// float2 + the CUDA 12.8+ sm_100 intrinsics, so ptxas allocates the aligned register pairs itself.
+// ---- fp32 pairs: Hopper has no packed FFMA2 / FMUL2 / FADD2, so each lane is one scalar round-to-nearest op ----
 typedef float2 zg_f2;
 __device__ __forceinline__ zg_f2 zg_pack2(float lo, float hi) { return make_float2(lo, hi); }
 __device__ __forceinline__ zg_f2 zg_splat2(float v) { return make_float2(v, v); }
-__device__ __forceinline__ zg_f2 zg_fma2(zg_f2 a, zg_f2 b, zg_f2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ zg_f2 zg_mul2(zg_f2 a, zg_f2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ zg_f2 zg_add2(zg_f2 a, zg_f2 b) { return __fadd2_rn(a, b); }
+__device__ __forceinline__ zg_f2 zg_fma2(zg_f2 a, zg_f2 b, zg_f2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ zg_f2 zg_mul2(zg_f2 a, zg_f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ zg_f2 zg_add2(zg_f2 a, zg_f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 // 2^x for two lanes at once via MUFU.EX2 (2 MUFU issues)
 __device__ __forceinline__ zg_f2 zg_ex2_mufu2(zg_f2 x) { return make_float2(zg_ex2(x.x), zg_ex2(x.y)); }
 // 2^x for two lanes on the FMA/ALU pipes only (no MUFU): Cody-Waite split x = i + f, |f| <= 0.5,

@@ -1,4 +1,4 @@
-"""Inference fast path of ZigMa.forward on B200: token-major, fused, CUDA-graph capturable.
+"""Inference fast path of ZigMa.forward on H100: token-major, fused, CUDA-graph capturable.
 
 What the reference executes per block (SURVEY.md section 3.2/3.3) and what replaces it here:
 
@@ -14,7 +14,7 @@ What the reference executes per block (SURVEY.md section 3.2/3.3) and what repla
 
 Numerics follow the reference's bf16 path rounding for rounding (every tensor the reference
 materialises in bf16 is rounded to bf16 at the same point), so results agree with the reference
-to fp32-accumulation-order noise.  The dense bf16 projections run on the hand-written tcgen05 kernel
+to fp32-accumulation-order noise.  The dense bf16 projections run on the hand-written wgmma kernel
 ``zg_gemm_bf16_tn`` (``ZIGMA_TCGEN05=0`` switches them to the library GEMM for A/B timing; fp32 models always
 use the library GEMM -- the tensor-core kernel is bf16 only).
 """
@@ -33,7 +33,7 @@ def _i32(t):
 
 
 def _linear(x2d, weight, bias=None):
-    """(M, K) @ (N, K)^T.  bf16 goes to the hand-written tcgen05 kernel (zg_gemm_bf16_tn; ZIGMA_TCGEN05=0 routes
+    """(M, K) @ (N, K)^T.  bf16 goes to the hand-written wgmma kernel (zg_gemm_bf16_tn; ZIGMA_TCGEN05=0, the switch's historical name, routes
     it to the library GEMM instead, e.g. for A/B timing); fp32 / fp16 always use the library GEMM."""
     if x2d.dtype == torch.bfloat16 and os.environ.get("ZIGMA_TCGEN05", "1") == "1" and x2d.stride(0) % 8 == 0 and weight.stride(0) % 8 == 0:
         from .gemm import linear_bf16
@@ -119,7 +119,7 @@ class ZigMaEngine:
         self._versions = None
         self._graphs = {}
         self.use_graph = os.environ.get("ZIGMA_CUDA_GRAPH", "1") != "0"
-        # dt_proj inside the scan kernel (zg_scan_params.dt_w): correct and tested, but measured SLOWER on B200 than GEMM + scan
+        # dt_proj inside the scan kernel (zg_scan_params.dt_w): correct and tested, but off by default (not measured on H100; it was slower than GEMM + scan where it was last measured)
         # (0.600 ms vs 0.507 + 0.042 ms per layer at config 2: the MMA + fragment epilogue lengthens the latency-bound
         # pre phase of every stage), so it is opt-in
         self.fuse_dt = os.environ.get("ZIGMA_FUSE_DT", "0") == "1"
@@ -200,7 +200,7 @@ class ZigMaEngine:
 
     def _patch_embed(self, x):
         """Patch embedding (model_zigma.py:608-614: a Conv2d with kernel = stride = patch, i.e. a per-patch linear map) as a GEMM
-        on the tcgen05 kernel: the K = C p^2 columns (4 at patch 1) are zero-padded to the 16-byte row pitch TMA needs.  Returns
+        on the wgmma kernel: the K = C p^2 columns (4 at patch 1) are zero-padded to the 16-byte row pitch TMA needs.  Returns
         (B, L, D) tokens, or None when the model is not bf16 (the module's own forward runs then)."""
         m = self.m
         if x.dtype != torch.bfloat16 or os.environ.get("ZIGMA_TCGEN05", "1") != "1":

@@ -1,4 +1,4 @@
-"""bf16 GEMM on tcgen05 tensor cores: ``linear_bf16(x, weight, bias)`` == ``F.linear`` for row-major
+"""bf16 GEMM on the Hopper tensor cores (wgmma): ``linear_bf16(x, weight, bias)`` == ``F.linear`` for row-major
 bf16 activations and an ``nn.Linear`` weight (N, K) -- the dense projections of the hot path
 (mamba_simple.py:290-294, selective_scan_interface.py:322-323,365).  C-ABI: zg_gemm_bf16_tn."""
 import torch

@@ -1,5 +1,5 @@
 """Host-side mirror of ``dis_mamba/mamba_ssm/ops/triton/layernorm.py`` (reference) over hand-written
-sm_100a kernels -- the reference launches Triton here; north_star forbids Triton on the hot path.
+sm_90a kernels -- the reference launches Triton here; north_star forbids Triton on the hot path.
 ``rms_norm_fn`` (:477-478), ``layer_norm_fn`` (:464-474), ``RMSNorm`` (:481-503), ``LayerNormFn``
 (:380-461)."""
 import torch

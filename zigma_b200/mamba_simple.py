@@ -1,5 +1,5 @@
 """ZigMa's Mamba mixer (``dis_mamba/mamba_ssm/modules/mamba_simple.py`` of the reference) on the
-sm_100a kernels.  Same constructor arguments, parameter names / shapes / init and scan-type
+sm_90a kernels.  Same constructor arguments, parameter names / shapes / init and scan-type
 dispatch (:64-268, :274-444); the single-token ``step`` / inference cache (:445-608) is out of
 scope (diffusion never decodes token by token).
 
@@ -45,7 +45,7 @@ class _PermuteFn(torch.autograd.Function):
     """y = x.index_select(dim, perm) for a PERMUTATION perm: the backward is the gather by the inverse
     permutation.  The reference writes ``x[:, :, perm]`` (mamba_simple.py:56,61), whose autograd
     backward is a sort-based index_put with accumulation -- 8 ms per layer at the config-2 shape,
-    46 % of a training step on B200 -- although no index repeats."""
+    a large share of a training step -- although no index repeats."""
 
     @staticmethod
     def forward(ctx, x, perm, inv, dim):

@@ -1,4 +1,4 @@
-"""ZigMa denoiser (``model_zigma.py`` of the reference) on the sm_100a kernels.
+"""ZigMa denoiser (``model_zigma.py`` of the reference) on the sm_90a kernels.
 
 Keeps the ``ZigMa(...)`` constructor (:549-576), ``forward(hidden_states, t, y=None)`` (:911-916) and
 the state-dict key layout (SURVEY.md section 8b) so reference checkpoints load unchanged.  Under
@@ -374,7 +374,7 @@ class ZigMa(nn.Module):
     # ---- forward ----------------------------------------------------------------------------------
     def embed(self, hidden_states, t, y=None, tokens=None, add_pos=True):
         """Everything before the blocks (model_zigma.py:923-947): tokens (B, L, D) and conditioning c.  ``tokens``: the
-        patch-embedding result when the caller computed it itself (the sampling engine runs that GEMM on its tcgen05 kernel)."""
+        patch-embedding result when the caller computed it itself (the sampling engine runs that GEMM on its wgmma kernel)."""
         hidden_states = self.x_embedder(hidden_states) if tokens is None else tokens
         _B = hidden_states.shape[0]
         t = self.t_embedder((t * 1000.0).to(hidden_states))

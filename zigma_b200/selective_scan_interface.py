@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's selective-scan op surface over the sm_100a kernels.
+"""Host-side mirror of the reference's selective-scan op surface over the sm_90a kernels.
 
 Same names, argument meaning and error behaviour as
 ``dis_mamba/mamba_ssm/ops/selective_scan_interface.py`` (reference):
@@ -431,7 +431,7 @@ class MambaInnerFn(torch.autograd.Function):
 # table; the backward scatters dx / dz rows back through the same table).  No transposed copies, no
 # index_select in either direction.
 def _tok_linear(x, w):
-    """x (M, K) @ w(N, K)^T on the tcgen05 kernel for bf16, cuBLAS otherwise."""
+    """x (M, K) @ w(N, K)^T on the wgmma kernel for bf16, cuBLAS otherwise."""
     if x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.is_cuda:
         from .engine import _linear
         return _linear(x, w)

@@ -5,7 +5,7 @@
     opt.zero_grad(); accelerator.backward(loss); opt.step()          # torch.optim.AdamW, DDP all-reduce inside backward
     grad_clip(opt, model, max_grad_norm); update_ema(ema_model, model)
 
--- laid out for a B200 node, one process per GPU:
+-- laid out for an H100 node, one process per GPU:
 
 * ``FlatParams``: every trainable parameter is a view into ONE flat fp32 buffer, every ``.grad`` a view into a
   second one (offsets 16-byte aligned).  zero_grad is one memset, the gradient norm one reduction, the

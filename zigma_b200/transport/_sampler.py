@@ -1,6 +1,6 @@
 """Transport / Sampler / sde / ode of the reference's ``transport/transport.py`` and
 ``transport/integrators.py`` -- the host-side loop that DRIVES the denoiser hot path (one or more
-``model(x, t, **kw)`` evaluations per step; each is one ZigMaEngine graph replay on the B200).
+``model(x, t, **kw)`` evaluations per step; each is one ZigMaEngine graph replay on the GPU).
 
 Random draws follow the reference exactly (what is drawn, in which order, from which generator:
 CPU ``torch.randn(x.size()).to(x)`` in the SDE steps, integrators.py:33,43; CPU ``torch.rand`` for
