@@ -267,6 +267,32 @@ typedef struct {
 int zg_block_tail_bwd(const zg_block_tail_bwd_params *p, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Deterministic backward (bitwise-identical outputs for bitwise-identical inputs on the same device and build, whatever
+ * order the CTAs run in; the Python layer calls these while torch.are_deterministic_algorithms_enabled()).
+ * Same params struct, outputs and zero-fill contract as the atomic twin above; the kernels are the same code compiled
+ * with every fp32 atomicAdd of a gradient reduction turned into a plain store into the value's own row of a partials
+ * workspace (the row follows from the static grid mapping: channel tile, warp, batch row or chunk index), and one
+ * reduction kernel then adds the rows into the outputs in row order (DESIGN.md section 4.6).
+ *   workspace:  device memory of at least zg_*_bwd_det_workspace_bytes(p) bytes, 16-byte aligned, no initial contents
+ *               needed; it must stay untouched until the call's work on `stream` is done.  A smaller workspace returns an
+ *               error (nothing is launched).
+ *   *_workspace_bytes: host arithmetic only (no GPU needed, no CUDA call), evaluated on the SAME params as the call: it
+ *               follows the kernel dispatch (dstate-16 vs generic scan kernel, token-major vs channel-first conv,
+ *               vectorised vs scalar norm, ...) and counts only the outputs that are not NULL.
+ * No allocation and no synchronisation inside: CUDA-graph capturable like the rest of the ABI.  The partial rows of
+ * zg_add_norm_bwd_det (one per CTA or warp, at most 528 CTAs) do not depend on the device; those of
+ * zg_block_tail_bwd_det follow p->nparts, so equal bits across devices need equal nparts.
+ * zg_block_tail_bwd_det additionally needs 4 * nparts >= batch (each warp stays inside one batch element). */
+int64_t zg_selective_scan_bwd_det_workspace_bytes(const zg_scan_bwd_params *p);
+int zg_selective_scan_bwd_det(const zg_scan_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+int64_t zg_causal_conv1d_bwd_det_workspace_bytes(const zg_conv_bwd_params *p);
+int zg_causal_conv1d_bwd_det(const zg_conv_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+int64_t zg_add_norm_bwd_det_workspace_bytes(const zg_norm_bwd_params *p);
+int zg_add_norm_bwd_det(const zg_norm_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+int64_t zg_block_tail_bwd_det_workspace_bytes(const zg_block_tail_bwd_params *p);
+int zg_block_tail_bwd_det(const zg_block_tail_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * bf16 GEMM on the Hopper tensor cores (wgmma):  C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]), fp32 accumulate in
  * registers, bf16 output.  A, B row-major with leading dims lda/ldb (elements, multiples of 8);
  * C row-major ldc.  out_rowmap (int32[rows_per_batch] or NULL): output row m of batch

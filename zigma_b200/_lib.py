@@ -94,6 +94,9 @@ class AdamWParams(C.Structure):
 EXPORTS = ["zg_abi_version", "zg_last_error", "zg_launch_count", "zg_last_scan_kernel", "zg_scan_kernel_choice", "zg_selective_scan_fwd", "zg_selective_scan_bwd",
            "zg_causal_conv1d_fwd", "zg_causal_conv1d_bwd", "zg_add_norm_fwd", "zg_add_norm_bwd",
            "zg_block_tail_fwd", "zg_block_tail_fwd_pe", "zg_block_tail_bwd", "zg_gemm_bf16_tn", "zg_adamw_ema_step"]
+# deterministic backward twins (zg_<op>_det + zg_<op>_det_workspace_bytes) of these entry points
+DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd"]
+EXPORTS += [n + s for n in DET_OPS for s in ("_det", "_det_workspace_bytes")]
 
 _lib = None
 
@@ -114,8 +117,15 @@ def lib():
         l.zg_scan_kernel_choice.restype = C.c_int
         l.zg_scan_kernel_choice.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         for name in EXPORTS[5:]:
-            getattr(l, name).restype = C.c_int
-            getattr(l, name).argtypes = [C.c_void_p, C.c_void_p]
+            if name.endswith("_det_workspace_bytes"):
+                getattr(l, name).restype = C.c_int64
+                getattr(l, name).argtypes = [C.c_void_p]
+            elif name.endswith("_det"):
+                getattr(l, name).restype = C.c_int
+                getattr(l, name).argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+            else:
+                getattr(l, name).restype = C.c_int
+                getattr(l, name).argtypes = [C.c_void_p, C.c_void_p]
         _lib = l
     return _lib
 
@@ -143,6 +153,26 @@ def call(name, params):
     rc = getattr(l, name)(C.byref(params), C.c_void_p(stream))
     if rc != 0:
         raise RuntimeError(f"{name}: {l.zg_last_error().decode()}")
+
+
+def det_workspace_bytes(name, params):
+    """Bytes of partials workspace the deterministic twin of backward entry point `name` needs for these params (host only)."""
+    return int(getattr(lib(), name + "_det_workspace_bytes")(C.byref(params)))
+
+
+def call_bwd(name, params):
+    """Invokes backward entry point `name` like ``call``; while ``torch.are_deterministic_algorithms_enabled()`` its
+    deterministic twin ``name + "_det"`` runs instead, with a partials workspace from torch's allocator on the current
+    device (the same gradients up to summation order, bitwise reproducible run to run)."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return call(name, params)
+    l = lib()
+    nbytes = det_workspace_bytes(name, params)
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=torch.device("cuda", torch.cuda.current_device()))
+    stream = torch.cuda.current_stream().cuda_stream
+    rc = getattr(l, name + "_det")(C.byref(params), C.c_void_p(ws.data_ptr() if nbytes else None), C.c_int64(nbytes), C.c_void_p(stream))
+    if rc != 0:
+        raise RuntimeError(f"{name}_det: {l.zg_last_error().decode()}")
 
 
 def dt(t):

@@ -63,7 +63,7 @@ class BlockTailFn(torch.autograd.Function):
         q.dgate, q.dshift, q.dscale, q.d_norm_w = (_lib.ptr(acc[0]) if mix is not None else None), _lib.ptr(acc[1]), _lib.ptr(acc[2]), _lib.ptr(d_w)
         q.mod_rs = scale.stride(0)
         q.batch, q.seqlen, q.dim, q.dtype, q.nparts = B, L, D, _lib.dt(act), nparts
-        _lib.call("zg_block_tail_bwd", q)
+        _lib.call_bwd("zg_block_tail_bwd", q)
         dt_mix, dt_gate, dt_shift, dt_scale = ctx.in_dtypes
         return (d_x, None if d_mix is None else d_mix.to(dt_mix), acc[0].to(dt_gate) if mix is not None else None,
                 acc[1].to(dt_shift or act), acc[2].to(dt_scale or act), d_w.sum(0).to(norm_w.dtype), d_res_in, None, None)

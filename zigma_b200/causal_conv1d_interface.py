@@ -87,7 +87,7 @@ def _conv_bwd(x, weight, bias, dout, silu, dx_out=None, x_rowmap=None):
     # `out` only takes part in the shared validation (layout class of the call)
     p.out = _lib.ptr(dx)
     p.out_sb, p.out_sd, p.out_sl = q.dx_sb, q.dx_sd, q.dx_sl
-    _lib.call("zg_causal_conv1d_bwd", q)
+    _lib.call_bwd("zg_causal_conv1d_bwd", q)
     return dx, dweight, dbias
 
 

@@ -28,7 +28,8 @@ int zg_check_launch(const char *what) {
 
 extern "C" {
 
-int zg_abi_version(void) { return 4; }   // 4: zg_block_tail_fwd_pe (positional embedding folded into the first tail)
+int zg_abi_version(void) { return 5; }   // 5: deterministic backward entry points zg_*_bwd_det + workspace queries
+// int zg_abi_version(void) { return 4; }   // 4: zg_block_tail_fwd_pe (positional embedding folded into the first tail)
 // int zg_abi_version(void) { return 3; }   // 3: fused dt_proj prologue fields in zg_scan_params
 // int zg_abi_version(void) { return 2; }   // 2: block-tail rstd + backward, AdamW+EMA step, (batch, n_ckpt, dim, dstate) checkpoints
 const char *zg_last_error(void) { return g_err; }

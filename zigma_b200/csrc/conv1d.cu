@@ -423,7 +423,9 @@ __global__ void __launch_bounds__(128) conv_fwd_seqc_kernel(const zg_conv_params
 // warp and accumulated with one fp32 atomicAdd per (row, tap).
 //   g[l]   = dout[l] * (silu ? silu'(pre[l]) : 1),  pre[l] = bias + sum_k w[k] x[l-k]
 //   dx[l]  = sum_k w[k] g[l+k]          dw[k] = sum_l g[l] x[l-k]        db = sum_l g[l]
-template <typename T>
+// DET (both channel-first kernels): dweight / dbias of q address partial rows, one per batch row -- (batch, dim, width) /
+// (batch, dim) -- stored, not added (zg_causal_conv1d_bwd_det).
+template <typename T, bool DET>
 __global__ void __launch_bounds__(128) conv_bwd_seqc_kernel(const zg_conv_bwd_params q) {
     const zg_conv_params &p = q.fwd;
     const int E = p.dim, L = p.seqlen, W = p.width;
@@ -460,7 +462,11 @@ __global__ void __launch_bounds__(128) conv_bwd_seqc_kernel(const zg_conv_bwd_pa
     db = zg_warp_sum(db);
 #pragma unroll
     for (int k = 0; k < 4; ++k) dw[k] = zg_warp_sum(dw[k]);
-    if (lane == 0) {
+    if (DET && lane == 0) {
+        const int64_t be = (int64_t)b * E + e;
+        if (q.dbias) q.dbias[be] = db;
+        for (int k = 0; k < W; ++k) q.dweight[be * W + (W - 1 - k)] = dw[k];
+    } else if (lane == 0) {
         if (q.dbias) atomicAdd(q.dbias + e, db);
         for (int k = 0; k < W; ++k) atomicAdd(q.dweight + (int64_t)e * W + (W - 1 - k), dw[k]);
     }
@@ -472,7 +478,7 @@ __global__ void __launch_bounds__(128) conv_bwd_seqc_kernel(const zg_conv_bwd_pa
 // x halo comes from the lane below and the g halo from the lane above by shuffles; tiles are walked from the
 // END of the row so that the three g values the last lane needs from the next tile are already known.  Each
 // silu' is evaluated once (the scalar kernel above evaluates it four times per position).
-template <typename T>
+template <typename T, bool DET>
 __global__ void __launch_bounds__(128) conv_bwd_seqc_vec_kernel(const zg_conv_bwd_params q) {
     constexpr int VEC = 16 / (int)sizeof(T);
     const zg_conv_params &p = q.fwd;
@@ -546,7 +552,11 @@ __global__ void __launch_bounds__(128) conv_bwd_seqc_vec_kernel(const zg_conv_bw
     db = zg_warp_sum(db);
 #pragma unroll
     for (int k = 0; k < 4; ++k) dw[k] = zg_warp_sum(dw[k]);
-    if (lane == 0) {
+    if (DET && lane == 0) {
+        const int64_t be = (int64_t)b * E + e;
+        if (q.dbias) q.dbias[be] = db;
+        for (int k = 0; k < W; ++k) q.dweight[be * W + (W - 1 - k)] = dw[k];
+    } else if (lane == 0) {
         if (q.dbias) atomicAdd(q.dbias + e, db);
         for (int k = 0; k < W; ++k) atomicAdd(q.dweight + (int64_t)e * W + (W - 1 - k), dw[k]);
     }
@@ -559,10 +569,12 @@ __global__ void __launch_bounds__(128) conv_bwd_seqc_vec_kernel(const zg_conv_bw
 // redirects both the x reads and the dx writes (the conv ran over the permuted sequence; dx goes
 // back to token order).  dweight/dbias: summed over the 4 warps of the CTA (4 chunks of the same
 // channels) in shared memory, then one atomic per (CTA, channel, tap).
+// DET (both token-major kernels): dweight / dbias of q address partial rows, one per CTA row group blockIdx.x / nvb
+// (= 4 consecutive (batch, chunk) rows) -- (ceil(batch * nchunk / 4), dim, width) / (.., dim) -- stored, not added.
 constexpr int CONV_BLCH = 64;
 constexpr int CONV_BRB = 4;     // rows per batch of independent loads in the backward (x and dout: 2 * CONV_BRB loads in flight)
 
-template <typename T, int DV, int BRB>
+template <typename T, int DV, int BRB, bool DET>
 __global__ void __launch_bounds__(128, (DV <= 2) ? 6 : 4) conv_bwd_tok_kernel(const zg_conv_bwd_params q) {
     const zg_conv_params &p = q.fwd;
     const int E = p.dim, L = p.seqlen, W = p.width;
@@ -681,8 +693,14 @@ __global__ void __launch_bounds__(128, (DV <= 2) ? 6 : 4) conv_bwd_tok_kernel(co
         if (vv >= nvec) continue;
         const float sum = red[0][j][ln] + red[1][j][ln] + red[2][j][ln] + red[3][j][ln];
         const int k = j / DV, i = j % DV, e = vv * DV + i;
-        if (k == 4) { if (q.dbias) atomicAdd(q.dbias + e, sum); }
-        else if (k < W) atomicAdd(q.dweight + (int64_t)e * W + (W - 1 - k), sum);
+        if constexpr (DET) {
+            const int64_t re = (int64_t)(blockIdx.x / nvb) * E + e;
+            if (k == 4) { if (q.dbias) q.dbias[re] = sum; }
+            else if (k < W) q.dweight[re * W + (W - 1 - k)] = sum;
+        } else {
+            if (k == 4) { if (q.dbias) atomicAdd(q.dbias + e, sum); }
+            else if (k < W) atomicAdd(q.dweight + (int64_t)e * W + (W - 1 - k), sum);
+        }
     }
 }
 
@@ -694,7 +712,7 @@ __global__ void __launch_bounds__(128, (DV <= 2) ? 6 : 4) conv_bwd_tok_kernel(co
 constexpr int CONV_B4_LCH = 32;
 constexpr int CONV_B4_RB = 4;
 
-template <typename T, bool HAS_MAP>
+template <typename T, bool HAS_MAP, bool DET>
 __global__ void __launch_bounds__(128, 4) conv_bwd_tok4_kernel(const zg_conv_bwd_params q) {
     static_assert(sizeof(T) == 2, "16-bit I/O");
     constexpr int LCH = CONV_B4_LCH, RB = CONV_B4_RB;
@@ -829,8 +847,14 @@ __global__ void __launch_bounds__(128, 4) conv_bwd_tok4_kernel(const zg_conv_bwd
         if (vv >= nvec) continue;
         const float sum = red[0][j][ln] + red[1][j][ln] + red[2][j][ln] + red[3][j][ln];
         const int k = j >> 2, i = j & 3, e = vv * 4 + i;
-        if (k == 4) { if (q.dbias) atomicAdd(q.dbias + e, sum); }
-        else if (k < W) atomicAdd(q.dweight + (int64_t)e * W + (W - 1 - k), sum);
+        if constexpr (DET) {
+            const int64_t re = (int64_t)(blockIdx.x / nvb) * E + e;
+            if (k == 4) { if (q.dbias) q.dbias[re] = sum; }
+            else if (k < W) q.dweight[re * W + (W - 1 - k)] = sum;
+        } else {
+            if (k == 4) { if (q.dbias) atomicAdd(q.dbias + e, sum); }
+            else if (k < W) atomicAdd(q.dweight + (int64_t)e * W + (W - 1 - k), sum);
+        }
     }
 }
 
@@ -940,34 +964,49 @@ extern "C" int zg_causal_conv1d_fwd(const zg_conv_params *pp, void *stream) {
     }
 }
 
-extern "C" int zg_causal_conv1d_bwd(const zg_conv_bwd_params *qq, void *stream) {
-    ZG_REQUIRE(qq != nullptr, "causal_conv1d_bwd: null params");
-    const zg_conv_bwd_params &q = *qq;
+// which backward kernel family runs a call (host arithmetic only; the launch and the deterministic workspace query share it)
+enum { CONV_BWD_TOK4 = 0, CONV_BWD_TOK = 1, CONV_BWD_SEQC = 2 };
+static int conv_bwd_kind(const zg_conv_bwd_params &q) {
+    const zg_conv_params &p = q.fwd;
+    if (!(p.x_sd == 1 && q.dout_sd == 1 && q.dx_sd == 1 && !(p.x_sl == 1 && p.dim > 1))) return CONV_BWD_SEQC;
+    const int esz = zg_dtype_size(p.dtype);
+    const uintptr_t al = reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(q.dout) | reinterpret_cast<uintptr_t>(q.dx);
+    const int64_t so = p.x_sb | p.x_sl | q.dout_sb | q.dout_sl | q.dx_sb | q.dx_sl;
+    const bool vec = (p.dim % 4 == 0) && (al % (4 * esz) == 0) && (so % 4 == 0);
+    static int fast4 = -1;             // ZG_CONV_BWD_FAST=0 disables the branch-free 16-bit kernel
+    if (fast4 < 0) { const char *e = getenv("ZG_CONV_BWD_FAST"); fast4 = e ? atoi(e) : 1; }
+    if (fast4 && esz == 2 && vec && p.seqlen % zg::CONV_B4_LCH == 0 && p.seqlen >= zg::CONV_B4_LCH &&
+        (int64_t)p.seqlen * p.x_sl < 0x7fffffffLL && (int64_t)p.seqlen * q.dout_sl < 0x7fffffffLL && (int64_t)p.seqlen * q.dx_sl < 0x7fffffffLL)
+        return CONV_BWD_TOK4;
+    return CONV_BWD_TOK;
+}
+
+static int conv_bwd_validate(const zg_conv_bwd_params &q) {
     if (int rc = conv_validate(q.fwd, "causal_conv1d_bwd")) return rc;
     ZG_REQUIRE(q.dout && q.dx && q.dweight, "causal_conv1d_bwd: null tensor pointer");
     ZG_REQUIRE(q.fwd.seg_len == 0, "causal_conv1d_bwd: seg_len is a forward (sampling) feature");
-    if (q.fwd.batch == 0 || q.fwd.seqlen == 0) return 0;
-    cudaStream_t s = (cudaStream_t)stream;
+    return 0;
+}
+
+template <bool DET> static int conv_bwd_launch(const zg_conv_bwd_params &q, cudaStream_t s) {
     const zg_conv_params &p = q.fwd;
-    if (p.x_sd == 1 && q.dout_sd == 1 && q.dx_sd == 1 && !(p.x_sl == 1 && p.dim > 1)) {
+    const int kind = conv_bwd_kind(q);
+    if (kind != CONV_BWD_SEQC) {
         // token-major: DV channels per thread when everything is DV-aligned
         const int esz = zg_dtype_size(p.dtype);
         const uintptr_t al = reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(q.dout) | reinterpret_cast<uintptr_t>(q.dx);
         const int64_t so = p.x_sb | p.x_sl | q.dout_sb | q.dout_sl | q.dx_sb | q.dx_sl;
         const bool vec = (p.dim % 4 == 0) && (al % (4 * esz) == 0) && (so % 4 == 0);
-        static int fast4 = -1;             // ZG_CONV_BWD_FAST=0 disables the branch-free 16-bit kernel
-        if (fast4 < 0) { const char *e = getenv("ZG_CONV_BWD_FAST"); fast4 = e ? atoi(e) : 1; }
-        if (fast4 && esz == 2 && vec && p.seqlen % zg::CONV_B4_LCH == 0 && p.seqlen >= zg::CONV_B4_LCH &&
-            (int64_t)p.seqlen * p.x_sl < 0x7fffffffLL && (int64_t)p.seqlen * q.dout_sl < 0x7fffffffLL && (int64_t)p.seqlen * q.dx_sl < 0x7fffffffLL) {
+        if (kind == CONV_BWD_TOK4) {
             const int nvb4 = (p.dim / 4 + 31) / 32;
             const int64_t g4 = (int64_t)nvb4 * (((int64_t)p.batch * (p.seqlen / zg::CONV_B4_LCH) + 3) / 4);
             ZG_REQUIRE(g4 <= 0x7fffffffLL, "causal_conv1d_bwd: grid too large");
             if (p.dtype == ZG_BF16) {
-                if (p.x_rowmap) zg::conv_bwd_tok4_kernel<__nv_bfloat16, true><<<(unsigned)g4, 128, 0, s>>>(q);
-                else zg::conv_bwd_tok4_kernel<__nv_bfloat16, false><<<(unsigned)g4, 128, 0, s>>>(q);
+                if (p.x_rowmap) zg::conv_bwd_tok4_kernel<__nv_bfloat16, true, DET><<<(unsigned)g4, 128, 0, s>>>(q);
+                else zg::conv_bwd_tok4_kernel<__nv_bfloat16, false, DET><<<(unsigned)g4, 128, 0, s>>>(q);
             } else {
-                if (p.x_rowmap) zg::conv_bwd_tok4_kernel<__half, true><<<(unsigned)g4, 128, 0, s>>>(q);
-                else zg::conv_bwd_tok4_kernel<__half, false><<<(unsigned)g4, 128, 0, s>>>(q);
+                if (p.x_rowmap) zg::conv_bwd_tok4_kernel<__half, true, DET><<<(unsigned)g4, 128, 0, s>>>(q);
+                else zg::conv_bwd_tok4_kernel<__half, false, DET><<<(unsigned)g4, 128, 0, s>>>(q);
             }
             zg_count_launch();
             return zg_check_launch("causal_conv1d_bwd(token-major, fast)");
@@ -982,11 +1021,11 @@ extern "C" int zg_causal_conv1d_bwd(const zg_conv_bwd_params *qq, void *stream) 
         ZG_REQUIRE(grid <= 0x7fffffffLL, "causal_conv1d_bwd: grid too large");
 #define ZG_CONV_BWD_TOK(TT)                                                                                  \
         do {                                                                                                 \
-            if (vec && dvs == 2 && brb == 4) zg::conv_bwd_tok_kernel<TT, 2, 4><<<(unsigned)grid, 128, 0, s>>>(q);      \
-            else if (vec && dvs == 2) zg::conv_bwd_tok_kernel<TT, 2, 8><<<(unsigned)grid, 128, 0, s>>>(q);             \
-            else if (vec && brb == 2) zg::conv_bwd_tok_kernel<TT, 4, 2><<<(unsigned)grid, 128, 0, s>>>(q);             \
-            else if (vec) zg::conv_bwd_tok_kernel<TT, 4, 4><<<(unsigned)grid, 128, 0, s>>>(q);                        \
-            else zg::conv_bwd_tok_kernel<TT, 1, 4><<<(unsigned)grid, 128, 0, s>>>(q);                                \
+            if (vec && dvs == 2 && brb == 4) zg::conv_bwd_tok_kernel<TT, 2, 4, DET><<<(unsigned)grid, 128, 0, s>>>(q);      \
+            else if (vec && dvs == 2) zg::conv_bwd_tok_kernel<TT, 2, 8, DET><<<(unsigned)grid, 128, 0, s>>>(q);             \
+            else if (vec && brb == 2) zg::conv_bwd_tok_kernel<TT, 4, 2, DET><<<(unsigned)grid, 128, 0, s>>>(q);             \
+            else if (vec) zg::conv_bwd_tok_kernel<TT, 4, 4, DET><<<(unsigned)grid, 128, 0, s>>>(q);                        \
+            else zg::conv_bwd_tok_kernel<TT, 1, 4, DET><<<(unsigned)grid, 128, 0, s>>>(q);                                \
         } while (0)
         switch (p.dtype) {
             case ZG_F32: ZG_CONV_BWD_TOK(float); break;
@@ -1006,10 +1045,50 @@ extern "C" int zg_causal_conv1d_bwd(const zg_conv_bwd_params *qq, void *stream) 
     const int64_t so2 = p.x_sb | p.x_sd | q.dout_sb | q.dout_sd | q.dx_sb | q.dx_sd;
     const bool fast = (p.seqlen % vec == 0) && (al2 % 16 == 0) && (so2 % vec == 0);
     switch (q.fwd.dtype) {
-        case ZG_F32: if (fast) zg::conv_bwd_seqc_vec_kernel<float><<<grid, 128, 0, s>>>(q); else zg::conv_bwd_seqc_kernel<float><<<grid, 128, 0, s>>>(q); break;
-        case ZG_F16: if (fast) zg::conv_bwd_seqc_vec_kernel<__half><<<grid, 128, 0, s>>>(q); else zg::conv_bwd_seqc_kernel<__half><<<grid, 128, 0, s>>>(q); break;
-        default: if (fast) zg::conv_bwd_seqc_vec_kernel<__nv_bfloat16><<<grid, 128, 0, s>>>(q); else zg::conv_bwd_seqc_kernel<__nv_bfloat16><<<grid, 128, 0, s>>>(q); break;
+        case ZG_F32: if (fast) zg::conv_bwd_seqc_vec_kernel<float, DET><<<grid, 128, 0, s>>>(q); else zg::conv_bwd_seqc_kernel<float, DET><<<grid, 128, 0, s>>>(q); break;
+        case ZG_F16: if (fast) zg::conv_bwd_seqc_vec_kernel<__half, DET><<<grid, 128, 0, s>>>(q); else zg::conv_bwd_seqc_kernel<__half, DET><<<grid, 128, 0, s>>>(q); break;
+        default: if (fast) zg::conv_bwd_seqc_vec_kernel<__nv_bfloat16, DET><<<grid, 128, 0, s>>>(q); else zg::conv_bwd_seqc_kernel<__nv_bfloat16, DET><<<grid, 128, 0, s>>>(q); break;
     }
     zg_count_launch();
     return zg_check_launch("causal_conv1d_bwd");
+}
+
+// partial-row regions of the deterministic backward (see the DET notes of the kernels): one row per batch row
+// (channel-first) or per 4 consecutive (batch, chunk) rows (token-major: 32-position chunks in the fast kernel, 64 otherwise)
+static ZgDetLayout conv_bwd_det_layout(const zg_conv_bwd_params &q, void *ws) {
+    const zg_conv_params &p = q.fwd;
+    ZgDetLayout lay;
+    lay.ws = static_cast<unsigned char *>(ws);
+    if (p.batch <= 0 || p.seqlen <= 0 || p.dim <= 0) return lay;
+    const int kind = conv_bwd_kind(q);
+    const int64_t rows = kind == CONV_BWD_SEQC ? p.batch
+                       : ((int64_t)p.batch * (kind == CONV_BWD_TOK4 ? p.seqlen / zg::CONV_B4_LCH : (p.seqlen + zg::CONV_BLCH - 1) / zg::CONV_BLCH) + 3) / 4;
+    lay.add(q.dweight, rows, (int64_t)p.dim * p.width);
+    lay.add(q.dbias, rows, p.dim);
+    return lay;
+}
+
+extern "C" int64_t zg_causal_conv1d_bwd_det_workspace_bytes(const zg_conv_bwd_params *q) {
+    return q ? conv_bwd_det_layout(*q, nullptr).bytes : 0;
+}
+
+extern "C" int zg_causal_conv1d_bwd_det(const zg_conv_bwd_params *qq, void *workspace, int64_t workspace_bytes, void *stream) {
+    ZG_REQUIRE(qq != nullptr, "causal_conv1d_bwd_det: null params");
+    if (int rc = conv_bwd_validate(*qq)) return rc;
+    if (qq->fwd.batch == 0 || qq->fwd.seqlen == 0) return 0;
+    const ZgDetLayout lay = conv_bwd_det_layout(*qq, workspace);
+    ZG_REQUIRE_WORKSPACE(lay, workspace, workspace_bytes, "causal_conv1d_bwd_det");
+    zg_conv_bwd_params q = *qq;                 // the kernel writes partial rows; the reduction adds them to the outputs
+    q.dweight = lay.reg[0].part;
+    if (q.dbias) q.dbias = lay.reg[1].part;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = conv_bwd_launch<true>(q, s)) return rc;
+    return lay.reduce(s);
+}
+
+extern "C" int zg_causal_conv1d_bwd(const zg_conv_bwd_params *qq, void *stream) {
+    ZG_REQUIRE(qq != nullptr, "causal_conv1d_bwd: null params");
+    if (int rc = conv_bwd_validate(*qq)) return rc;
+    if (qq->fwd.batch == 0 || qq->fwd.seqlen == 0) return 0;
+    return conv_bwd_launch<false>(*qq, (cudaStream_t)stream);
 }

@@ -128,7 +128,9 @@ __global__ void __launch_bounds__(128) add_norm_fwd_kernel(const zg_norm_params 
 // dw/db accumulated per CTA in shared memory then atomically into the fp32 outputs.
 //   xhat = (x - mean) * rstd;  wdy = dy * w;  c1 = mean(xhat * wdy);  c2 = mean(wdy) (0 for RMS)
 //   dx = (wdy - (xhat * c1 + c2)) * rstd (+ dresidual)
-template <typename T, typename R>
+// DET: dweight / dbias of p address partial rows, one per warp of the grid -- (gridDim.x * 4, ncols) -- stored, not added
+// (zg_add_norm_bwd_det).
+template <typename T, typename R, bool DET>
 __global__ void __launch_bounds__(128) add_norm_bwd_kernel(const zg_norm_bwd_params p) {
     // persistent warps: each warp walks rows with a grid stride and keeps its dweight/dbias partial
     // sums in registers (lane owns columns lane, lane+32, ...), one atomicAdd per column at the end.
@@ -176,7 +178,10 @@ __global__ void __launch_bounds__(128) add_norm_bwd_kernel(const zg_norm_bwd_par
 #pragma unroll
     for (int k = 0; k < MAXC; ++k) {
         const int i = lane + 32 * k;
-        if (i < N) {
+        if (DET && i < N) {
+            if (p.dweight) p.dweight[(int64_t)warp * N + i] = dw[k];
+            if (p.dbias) p.dbias[(int64_t)warp * N + i] = db[k];
+        } else if (i < N) {
             if (p.dweight) atomicAdd(p.dweight + i, dw[k]);
             if (p.dbias) atomicAdd(p.dbias + i, db[k]);
         }
@@ -189,7 +194,8 @@ __global__ void __launch_bounds__(128) add_norm_bwd_kernel(const zg_norm_bwd_par
 // shared memory before the atomics.  (The scalar kernel below remains for unaligned / odd shapes: ncu
 // round 1 had it at 0.36 ms for 16384 x 640 -- 2-byte loads, 128 accumulator registers, two dependent
 // passes over global memory -- against 0.03 ms of HBM time.)
-template <typename T, typename R, int MAXQ>
+// DET: dweight / dbias of p address partial rows, one per CTA -- (gridDim.x, ncols) -- stored, not added.
+template <typename T, typename R, int MAXQ, bool DET>
 __global__ void __launch_bounds__(128) add_norm_bwd_vec_kernel(const zg_norm_bwd_params p) {
     const int warp = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int nwarps = (int)(((int64_t)gridDim.x * blockDim.x) >> 5);
@@ -269,7 +275,11 @@ __global__ void __launch_bounds__(128) add_norm_bwd_vec_kernel(const zg_norm_bwd
             for (int i = 0; i < 4; ++i) red[wib][4 * (lane + 32 * k) + i] = pass ? db[k][i] : dw[k][i];
         __syncthreads();
         float *dst = pass ? p.dbias : p.dweight;
-        for (int c = threadIdx.x; c < N; c += 128) atomicAdd(dst + c, red[0][c] + red[1][c] + red[2][c] + red[3][c]);
+        if constexpr (DET) {
+            for (int c = threadIdx.x; c < N; c += 128) dst[(int64_t)blockIdx.x * N + c] = red[0][c] + red[1][c] + red[2][c] + red[3][c];
+        } else {
+            for (int c = threadIdx.x; c < N; c += 128) atomicAdd(dst + c, red[0][c] + red[1][c] + red[2][c] + red[3][c]);
+        }
     }
 }
 
@@ -602,7 +612,11 @@ template <typename T> static int block_tail_t(const zg_block_tail_params &p, cud
 // read once as raw 8/16-byte vectors; 22 B read + 10 B written per element (bf16), pure HBM streaming.
 constexpr int TAILB_ROWS = 16;
 
-template <typename T, int MAXQ>
+// DET: warps are partitioned per batch element instead -- wpb = nwarps / batch warps per element, warp w takes an equal
+// contiguous share of the rows of element w / wpb (warps past batch * wpb idle) -- so that a warp never crosses a batch
+// boundary; dgate / dshift / dscale of p address partial rows, one per warp index within the element, (wpb, batch, dim),
+// stored (zeros for a warp without rows), not added (zg_block_tail_bwd_det).  d_norm_w is the same partials buffer in both.
+template <typename T, int MAXQ, bool DET>
 __global__ void __launch_bounds__(128, 3) block_tail_bwd_kernel(const zg_block_tail_bwd_params p) {
     // per-batch column sums live in shared memory (lane-private slots, no conflicts): keeping all four accumulator sets
     // in registers cost 212 registers = 8 warps per SM, too few for a streaming kernel
@@ -637,7 +651,9 @@ __global__ void __launch_bounds__(128, 3) block_tail_bwd_kernel(const zg_block_t
 #pragma unroll
                 for (int j = 0; j < 3; ++j) {
                     const float4 v = acc_s[(j * MAXQ + k) * 32];
-                    if (dst[j]) {
+                    if (DET && dst[j]) {
+                        *reinterpret_cast<float4 *>(dst[j] + ((warp % (nwarps / p.batch)) * p.batch + b) * D + 4 * q) = v;
+                    } else if (dst[j]) {
                         float *o = dst[j] + (int64_t)b * D + 4 * q;
                         atomicAdd(o, v.x); atomicAdd(o + 1, v.y); atomicAdd(o + 2, v.z); atomicAdd(o + 3, v.w);
                     }
@@ -646,7 +662,16 @@ __global__ void __launch_bounds__(128, 3) block_tail_bwd_kernel(const zg_block_t
             }
         }
     };
-    const int64_t row0 = min(warp * per, nrows), row1 = min(row0 + per, nrows);
+    int64_t row0 = min(warp * per, nrows), row1 = min(row0 + per, nrows);
+    if constexpr (DET) {
+        const int64_t wpb = nwarps / p.batch, bw = warp / wpb, per_b = (p.seqlen + wpb - 1) / wpb;
+        row0 = row1 = nrows;
+        if (bw < p.batch) {
+            row0 = bw * p.seqlen + min((warp % wpb) * per_b, (int64_t)p.seqlen);
+            row1 = bw * p.seqlen + min((warp % wpb + 1) * per_b, (int64_t)p.seqlen);
+            if (row0 == row1) flush_batch((int)bw);      // no rows: this warp's partial rows are zeros
+        }
+    }
     if (row0 < row1) {
     int cur_b = (int)(row0 / p.seqlen);
     for (int64_t row = row0; row < row1; ++row) {
@@ -758,13 +783,13 @@ __global__ void __launch_bounds__(128, 3) block_tail_bwd_kernel(const zg_block_t
     }
 }
 
-template <typename T> static int block_tail_bwd_t(const zg_block_tail_bwd_params &p, cudaStream_t s) {
+template <typename T, bool DET> static int block_tail_bwd_t(const zg_block_tail_bwd_params &p, cudaStream_t s) {
     const unsigned grid = (unsigned)p.nparts;          // persistent: the caller sized the d_norm_w partials buffer
     // dynamic shared memory: 4 warps x 3 accumulator sets x MAXQ quads x 32 lanes x 16 B  (<= 48 KB for MAXQ <= 8)
-    if (p.dim <= 512) block_tail_bwd_kernel<T, 4><<<grid, 128, 4 * 3 * 4 * 32 * 16, s>>>(p);
-    else if (p.dim <= 640) block_tail_bwd_kernel<T, 5><<<grid, 128, 4 * 3 * 5 * 32 * 16, s>>>(p);
-    else if (p.dim <= 768) block_tail_bwd_kernel<T, 6><<<grid, 128, 4 * 3 * 6 * 32 * 16, s>>>(p);
-    else block_tail_bwd_kernel<T, 8><<<grid, 128, 4 * 3 * 8 * 32 * 16, s>>>(p);
+    if (p.dim <= 512) block_tail_bwd_kernel<T, 4, DET><<<grid, 128, 4 * 3 * 4 * 32 * 16, s>>>(p);
+    else if (p.dim <= 640) block_tail_bwd_kernel<T, 5, DET><<<grid, 128, 4 * 3 * 5 * 32 * 16, s>>>(p);
+    else if (p.dim <= 768) block_tail_bwd_kernel<T, 6, DET><<<grid, 128, 4 * 3 * 6 * 32 * 16, s>>>(p);
+    else block_tail_bwd_kernel<T, 8, DET><<<grid, 128, 4 * 3 * 8 * 32 * 16, s>>>(p);
     zg_count_launch();
     return zg_check_launch("block_tail_bwd");
 }
@@ -780,29 +805,37 @@ template <typename T> static int norm_fwd_t(const zg_norm_params &p, cudaStream_
     if (p.res_dtype == p.dtype) return norm_fwd_tr<T, T>(p, s);
     return zg_set_error("add_norm_fwd: residual dtype must be fp32 or the activation dtype");
 }
-template <typename T, typename R> static int norm_bwd_tr(const zg_norm_bwd_params &p, cudaStream_t s) {
+// launch shape of the backward (host arithmetic only; the launch and the deterministic workspace query share it):
+// CTAs (at most 528, whatever the SM count) and whether the vectorised kernel runs
+static unsigned norm_bwd_grid(const zg_norm_bwd_params &p) {
     const int64_t want = ((int64_t)p.nrows * 32 + 127) / 128;
-    const unsigned grid = (unsigned)(want < 132 * 4 ? want : 132 * 4);
+    return (unsigned)(want < 132 * 4 ? want : 132 * 4);
+}
+static bool norm_bwd_vec(const zg_norm_bwd_params &p) {
     const uintptr_t al = reinterpret_cast<uintptr_t>(p.dy) | reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(p.dresidual) |
                          reinterpret_cast<uintptr_t>(p.dx) | reinterpret_cast<uintptr_t>(p.dresidual_in);
     const int64_t so = p.dy_rs | p.x_rs | p.dx_rs | (p.dresidual ? p.dres_rs : 0) | (p.dresidual_in ? p.dresin_rs : 0);
-    if (p.ncols % 4 == 0 && al % 16 == 0 && so % 4 == 0 && p.ncols <= 1024) {
+    return p.ncols % 4 == 0 && al % 16 == 0 && so % 4 == 0 && p.ncols <= 1024;
+}
+template <typename T, typename R, bool DET> static int norm_bwd_tr(const zg_norm_bwd_params &p, cudaStream_t s) {
+    const unsigned grid = norm_bwd_grid(p);
+    if (norm_bwd_vec(p)) {
         const int nq = p.ncols / 4;
-        if (nq <= 32 * 2) add_norm_bwd_vec_kernel<T, R, 2><<<grid, 128, 0, s>>>(p);
-        else if (nq <= 32 * 4) add_norm_bwd_vec_kernel<T, R, 4><<<grid, 128, 0, s>>>(p);
-        else if (nq <= 32 * 5) add_norm_bwd_vec_kernel<T, R, 5><<<grid, 128, 0, s>>>(p);
-        else if (nq <= 32 * 6) add_norm_bwd_vec_kernel<T, R, 6><<<grid, 128, 0, s>>>(p);
-        else add_norm_bwd_vec_kernel<T, R, 8><<<grid, 128, 0, s>>>(p);
+        if (nq <= 32 * 2) add_norm_bwd_vec_kernel<T, R, 2, DET><<<grid, 128, 0, s>>>(p);
+        else if (nq <= 32 * 4) add_norm_bwd_vec_kernel<T, R, 4, DET><<<grid, 128, 0, s>>>(p);
+        else if (nq <= 32 * 5) add_norm_bwd_vec_kernel<T, R, 5, DET><<<grid, 128, 0, s>>>(p);
+        else if (nq <= 32 * 6) add_norm_bwd_vec_kernel<T, R, 6, DET><<<grid, 128, 0, s>>>(p);
+        else add_norm_bwd_vec_kernel<T, R, 8, DET><<<grid, 128, 0, s>>>(p);
         zg_count_launch();
         return zg_check_launch("add_norm_bwd(vec)");
     }
-    add_norm_bwd_kernel<T, R><<<grid, 128, 0, s>>>(p);
+    add_norm_bwd_kernel<T, R, DET><<<grid, 128, 0, s>>>(p);
     zg_count_launch();
     return zg_check_launch("add_norm_bwd");
 }
-template <typename T> static int norm_bwd_t(const zg_norm_bwd_params &p, cudaStream_t s) {
-    if (p.res_dtype == ZG_F32) return norm_bwd_tr<T, float>(p, s);
-    if (p.res_dtype == p.dtype) return norm_bwd_tr<T, T>(p, s);
+template <typename T, bool DET> static int norm_bwd_t(const zg_norm_bwd_params &p, cudaStream_t s) {
+    if (p.res_dtype == ZG_F32) return norm_bwd_tr<T, float, DET>(p, s);
+    if (p.res_dtype == p.dtype) return norm_bwd_tr<T, T, DET>(p, s);
     return zg_set_error("add_norm_bwd: residual dtype must be fp32 or the activation dtype");
 }
 
@@ -828,19 +861,56 @@ extern "C" int zg_add_norm_fwd(const zg_norm_params *pp, void *stream) {
     return zg_set_error("add_norm_fwd: bad dtype %d", p.dtype);
 }
 
-extern "C" int zg_add_norm_bwd(const zg_norm_bwd_params *pp, void *stream) {
-    ZG_REQUIRE(pp != nullptr, "add_norm_bwd: null params");
-    const zg_norm_bwd_params &p = *pp;
+static int norm_bwd_validate(const zg_norm_bwd_params &p) {
     ZG_REQUIRE(p.dy && p.x && p.dx && p.rstd, "add_norm_bwd: null tensor pointer");
     ZG_REQUIRE(p.ncols > 0 && p.ncols <= 4 * 32 * zg::NORM_MAXQ, "add_norm_bwd: ncols must be <= %d, got %d", 4 * 32 * zg::NORM_MAXQ, p.ncols);
-    if (p.nrows == 0) return 0;
-    cudaStream_t s = (cudaStream_t)stream;
+    ZG_REQUIRE(p.dtype == ZG_F32 || p.dtype == ZG_F16 || p.dtype == ZG_BF16, "add_norm_bwd: bad dtype %d", p.dtype);
+    return 0;
+}
+
+template <bool DET> static int norm_bwd_dispatch(const zg_norm_bwd_params &p, cudaStream_t s) {
     switch (p.dtype) {
-        case ZG_F32: return zg::norm_bwd_t<float>(p, s);
-        case ZG_F16: return zg::norm_bwd_t<__half>(p, s);
-        case ZG_BF16: return zg::norm_bwd_t<__nv_bfloat16>(p, s);
+        case ZG_F32: return zg::norm_bwd_t<float, DET>(p, s);
+        case ZG_F16: return zg::norm_bwd_t<__half, DET>(p, s);
+        default: return zg::norm_bwd_t<__nv_bfloat16, DET>(p, s);
     }
-    return zg_set_error("add_norm_bwd: bad dtype %d", p.dtype);
+}
+
+extern "C" int zg_add_norm_bwd(const zg_norm_bwd_params *pp, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "add_norm_bwd: null params");
+    if (int rc = norm_bwd_validate(*pp)) return rc;
+    if (pp->nrows == 0) return 0;
+    return norm_bwd_dispatch<false>(*pp, (cudaStream_t)stream);
+}
+
+// partial rows of the deterministic backward: one per CTA (vectorised kernel) or per warp (scalar kernel)
+static ZgDetLayout norm_bwd_det_layout(const zg_norm_bwd_params &p, void *ws) {
+    ZgDetLayout lay;
+    lay.ws = static_cast<unsigned char *>(ws);
+    if (p.nrows <= 0 || p.ncols <= 0) return lay;
+    const int64_t rows = (int64_t)zg::norm_bwd_grid(p) * (zg::norm_bwd_vec(p) ? 1 : 4);
+    lay.add(p.dweight, rows, p.ncols);
+    lay.add(p.dbias, rows, p.ncols);
+    return lay;
+}
+
+extern "C" int64_t zg_add_norm_bwd_det_workspace_bytes(const zg_norm_bwd_params *p) {
+    return p ? norm_bwd_det_layout(*p, nullptr).bytes : 0;
+}
+
+extern "C" int zg_add_norm_bwd_det(const zg_norm_bwd_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "add_norm_bwd_det: null params");
+    if (int rc = norm_bwd_validate(*pp)) return rc;
+    if (pp->nrows == 0) return 0;
+    const ZgDetLayout lay = norm_bwd_det_layout(*pp, workspace);
+    ZG_REQUIRE_WORKSPACE(lay, workspace, workspace_bytes, "add_norm_bwd_det");
+    zg_norm_bwd_params p = *pp;                 // the kernel writes partial rows; the reduction adds them to the outputs
+    int i = 0;
+    if (p.dweight) p.dweight = lay.reg[i++].part;
+    if (p.dbias) p.dbias = lay.reg[i++].part;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = norm_bwd_dispatch<true>(p, s)) return rc;
+    return lay.reduce(s);
 }
 
 static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bool pe) {
@@ -869,9 +939,7 @@ static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bo
 extern "C" int zg_block_tail_fwd(const zg_block_tail_params *pp, void *stream) { return block_tail_fwd_entry(pp, stream, false); }
 extern "C" int zg_block_tail_fwd_pe(const zg_block_tail_params *pp, void *stream) { return block_tail_fwd_entry(pp, stream, true); }
 
-extern "C" int zg_block_tail_bwd(const zg_block_tail_bwd_params *pp, void *stream) {
-    ZG_REQUIRE(pp != nullptr, "block_tail_bwd: null params");
-    const zg_block_tail_bwd_params &p = *pp;
+static int block_tail_bwd_validate(const zg_block_tail_bwd_params &p) {
     ZG_REQUIRE(p.r && p.rstd && p.norm_w && p.d_x, "block_tail_bwd: null tensor pointer");
     ZG_REQUIRE((p.mix != nullptr) == (p.gate != nullptr) && (p.mix != nullptr) == (p.d_mix != nullptr), "block_tail_bwd: mix, gate and d_mix go together");
     ZG_REQUIRE(!p.d_modded || p.scale, "block_tail_bwd: d_modded needs scale");
@@ -881,12 +949,55 @@ extern "C" int zg_block_tail_bwd(const zg_block_tail_bwd_params *pp, void *strea
     ZG_REQUIRE(aligned16(p.r) && aligned16(p.d_residual_out) && aligned16(p.d_normed) && aligned16(p.d_modded) && aligned16(p.mix) && aligned16(p.d_x) &&
                    aligned16(p.d_mix) && aligned16(p.d_residual_in) && aligned16(p.gate) && aligned16(p.scale) && aligned16(p.norm_w),
                "block_tail_bwd: tensors must be 16-byte aligned");
-    if (p.batch == 0 || p.seqlen == 0) return 0;
-    cudaStream_t s = (cudaStream_t)stream;
+    ZG_REQUIRE(p.dtype == ZG_F32 || p.dtype == ZG_F16 || p.dtype == ZG_BF16, "block_tail_bwd: bad dtype %d", p.dtype);
+    return 0;
+}
+
+template <bool DET> static int block_tail_bwd_dispatch(const zg_block_tail_bwd_params &p, cudaStream_t s) {
     switch (p.dtype) {
-        case ZG_F32: return zg::block_tail_bwd_t<float>(p, s);
-        case ZG_F16: return zg::block_tail_bwd_t<__half>(p, s);
-        case ZG_BF16: return zg::block_tail_bwd_t<__nv_bfloat16>(p, s);
+        case ZG_F32: return zg::block_tail_bwd_t<float, DET>(p, s);
+        case ZG_F16: return zg::block_tail_bwd_t<__half, DET>(p, s);
+        default: return zg::block_tail_bwd_t<__nv_bfloat16, DET>(p, s);
     }
-    return zg_set_error("block_tail_bwd: bad dtype %d", p.dtype);
+}
+
+extern "C" int zg_block_tail_bwd(const zg_block_tail_bwd_params *pp, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_bwd: null params");
+    if (int rc = block_tail_bwd_validate(*pp)) return rc;
+    if (pp->batch == 0 || pp->seqlen == 0) return 0;
+    return block_tail_bwd_dispatch<false>(*pp, (cudaStream_t)stream);
+}
+
+// partial rows of the deterministic backward: one per warp index within a batch element (see block_tail_bwd_kernel)
+static ZgDetLayout block_tail_bwd_det_layout(const zg_block_tail_bwd_params &p, void *ws) {
+    ZgDetLayout lay;
+    lay.ws = static_cast<unsigned char *>(ws);
+    if (p.batch <= 0 || p.seqlen <= 0 || p.dim <= 0 || p.nparts < 1) return lay;
+    const int64_t wpb = 4 * (int64_t)p.nparts / p.batch, n = (int64_t)p.batch * p.dim;
+    lay.add(p.dgate, wpb, n);
+    lay.add(p.dshift, wpb, n);
+    lay.add(p.dscale, wpb, n);
+    return lay;
+}
+
+extern "C" int64_t zg_block_tail_bwd_det_workspace_bytes(const zg_block_tail_bwd_params *p) {
+    return p ? block_tail_bwd_det_layout(*p, nullptr).bytes : 0;
+}
+
+extern "C" int zg_block_tail_bwd_det(const zg_block_tail_bwd_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_bwd_det: null params");
+    if (int rc = block_tail_bwd_validate(*pp)) return rc;
+    if (pp->batch == 0 || pp->seqlen == 0) return 0;
+    ZG_REQUIRE(4 * (int64_t)pp->nparts >= pp->batch, "block_tail_bwd_det: needs at least one warp per batch element (4 * nparts >= batch), got nparts %d for batch %d",
+               pp->nparts, pp->batch);
+    const ZgDetLayout lay = block_tail_bwd_det_layout(*pp, workspace);
+    ZG_REQUIRE_WORKSPACE(lay, workspace, workspace_bytes, "block_tail_bwd_det");
+    zg_block_tail_bwd_params p = *pp;           // the kernel writes partial rows; the reduction adds them to the outputs
+    int i = 0;
+    if (p.dgate) p.dgate = lay.reg[i++].part;
+    if (p.dshift) p.dshift = lay.reg[i++].part;
+    if (p.dscale) p.dscale = lay.reg[i++].part;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = block_tail_bwd_dispatch<true>(p, s)) return rc;
+    return lay.reduce(s);
 }

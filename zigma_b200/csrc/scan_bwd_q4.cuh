@@ -54,7 +54,10 @@ template <> __device__ __forceinline__ void q4_st_pair<__nv_bfloat16>(__nv_bfloa
     *reinterpret_cast<__nv_bfloat162 *>(p) = __floats2bfloat162_rn(a, b);
 }
 
-template <typename T, bool STAGED>
+// DET: the gradient pointers of q address partial rows instead of the outputs (zg_selective_scan_bwd_det): dB / dC one
+// row per channel tile within the group, (tiles_per_group, batch, groups, 16, seqlen); dA / dD / d(delta_bias) one row per
+// batch row, (batch, dim, 16) / (batch, dim); plain stores where the atomic path adds.
+template <typename T, bool STAGED, bool DET>
 __global__ void __launch_bounds__(Q4_THREADS, 4) scan_bwd_q4_kernel(const zg_scan_bwd_params q) {
     const zg_scan_params &p = q.fwd;
     constexpr int TS = Q4_TS, CH = Q4_CH;
@@ -114,8 +117,9 @@ __global__ void __launch_bounds__(Q4_THREADS, 4) scan_bwd_q4_kernel(const zg_sca
     T *gdu = reinterpret_cast<T *>(q.du) + (int64_t)b * q.du_sb + (int64_t)e0 * q.du_sd;
     T *gdd = reinterpret_cast<T *>(q.ddelta) + (int64_t)b * q.ddelta_sb + (int64_t)e0 * q.ddelta_sd;
     T *gdz = has_z ? reinterpret_cast<T *>(q.dz) + (int64_t)b * q.dz_sb + (int64_t)e0 * q.dz_sd : nullptr;
-    float *gdB = q.dB + ((int64_t)b * p.ngroups + g) * (int64_t)16 * L;      // (batch, groups, dstate, seqlen)
-    float *gdC = q.dC + ((int64_t)b * p.ngroups + g) * (int64_t)16 * L;
+    const int64_t det_row = DET ? (int64_t)(tile % tiles_per_group) * p.batch * p.ngroups * 16 * L : 0;
+    float *gdB = q.dB + det_row + ((int64_t)b * p.ngroups + g) * (int64_t)16 * L;      // (batch, groups, dstate, seqlen)
+    float *gdC = q.dC + det_row + ((int64_t)b * p.ngroups + g) * (int64_t)16 * L;
     const int nck = (L + TS - 1) / TS;
     const float4 *ck = reinterpret_cast<const float4 *>(p.ckpt + ((int64_t)b * nck * E + e) * (int64_t)16) + qd;   // (batch, n_ckpt, dim, 16)
     // B / C: 2 x 8 steps x 16 states = 256 values, one per thread
@@ -343,12 +347,23 @@ __global__ void __launch_bounds__(Q4_THREADS, 4) scan_bwd_q4_kernel(const zg_sca
             float acc = 0.f;
 #pragma unroll
             for (int w = 0; w < 8; ++w) acc += red[(w * 32 + slot) * Q4_RED_LD + t];
-            if (l < L) atomicAdd((slot < 16 ? gdB : gdC) + (int64_t)(slot & 15) * L + l, acc);
+            if (l < L) {
+                float *dst = (slot < 16 ? gdB : gdC) + (int64_t)(slot & 15) * L + l;
+                if constexpr (DET) *dst = acc;
+                else atomicAdd(dst, acc);
+            }
         }
         if (!STAGED) __syncthreads();      // (STAGED: the barrier at the top of the next iteration does this job)
     }
 
-    if (active) {
+    if (DET && active) {
+        const int64_t be = (int64_t)b * E + e;
+        *reinterpret_cast<float4 *>(q.dA + be * 16 + 4 * qd) = make_float4(dA[0].x, dA[0].y, dA[1].x, dA[1].y);
+        if (qd == 0) {
+            if (q.dD) q.dD[be] = dD_acc;
+            if (q.ddelta_bias) q.ddelta_bias[be] = dbias_acc;
+        }
+    } else if (active) {
         float *dAe = q.dA + (int64_t)e * 16 + 4 * qd;
         atomicAdd(dAe + 0, dA[0].x); atomicAdd(dAe + 1, dA[0].y);
         atomicAdd(dAe + 2, dA[1].x); atomicAdd(dAe + 3, dA[1].y);
@@ -359,18 +374,27 @@ __global__ void __launch_bounds__(Q4_THREADS, 4) scan_bwd_q4_kernel(const zg_sca
     }
 }
 
-// returns -1 when the call does not fit this specialisation
-template <typename T> int try_launch_scan_bwd_q4(const zg_scan_bwd_params &q, cudaStream_t s) {
-    static int enabled = -1, staged_ok = -1;
+// whether a call runs the dstate == 16 kernel (else the generic one in scan_bwd.cu); host arithmetic only
+static inline bool scan_bwd_q4_fits(const zg_scan_bwd_params &q) {
+    static int enabled = -1;
     if (enabled < 0) { const char *e = getenv("ZG_SCAN_BWD_Q4"); enabled = e ? atoi(e) : 1; }
-    if (staged_ok < 0) { const char *e = getenv("ZG_SCAN_BWD_STAGED"); staged_ok = e ? atoi(e) : 1; }
     const zg_scan_params &p = q.fwd;
-    if (!enabled || p.dstate != 16 || p.ckpt_every != Q4_TS) return -1;
-    if (!(p.flags & ZG_SCAN_VARIABLE_B) || !(p.flags & ZG_SCAN_VARIABLE_C)) return -1;      // constant B / C: the generic kernel
-    if ((reinterpret_cast<uintptr_t>(p.A) | reinterpret_cast<uintptr_t>(p.ckpt)) % 16 != 0) return -1;
+    if (!enabled || p.dstate != 16 || p.ckpt_every != Q4_TS) return false;
+    if (!(p.flags & ZG_SCAN_VARIABLE_B) || !(p.flags & ZG_SCAN_VARIABLE_C)) return false;      // constant B / C: the generic kernel
+    if ((reinterpret_cast<uintptr_t>(p.A) | reinterpret_cast<uintptr_t>(p.ckpt)) % 16 != 0) return false;
     const int per_group = p.dim / p.ngroups;
     const long long nblk = (long long)p.ngroups * ((per_group + Q4_CH - 1) / Q4_CH) * p.batch;
-    if (nblk > 0x7fffffffLL) return -1;
+    return nblk <= 0x7fffffffLL;
+}
+
+// returns -1 when the call does not fit this specialisation
+template <typename T, bool DET = false> int try_launch_scan_bwd_q4(const zg_scan_bwd_params &q, cudaStream_t s) {
+    static int staged_ok = -1;
+    if (staged_ok < 0) { const char *e = getenv("ZG_SCAN_BWD_STAGED"); staged_ok = e ? atoi(e) : 1; }
+    if (!scan_bwd_q4_fits(q)) return -1;
+    const zg_scan_params &p = q.fwd;
+    const int per_group = p.dim / p.ngroups;
+    const long long nblk = (long long)p.ngroups * ((per_group + Q4_CH - 1) / Q4_CH) * p.batch;
 
     // staged variant: whole tiles and chunks, one layout for all activations, 16-byte aligned rows, 32-bit offsets
     constexpr int EPC = 16 / (int)sizeof(T);
@@ -404,8 +428,8 @@ template <typename T> int try_launch_scan_bwd_q4(const zg_scan_bwd_params &q, cu
         zg_count_launch();
         return zg_check_launch("scan_bwd(q4)");
     };
-    if (staged) return launch(scan_bwd_q4_kernel<T, true>, Q4Smem<T, true>::TOTAL);
-    return launch(scan_bwd_q4_kernel<T, false>, Q4Smem<T, false>::TOTAL);
+    if (staged) return launch(scan_bwd_q4_kernel<T, true, DET>, Q4Smem<T, true>::TOTAL);
+    return launch(scan_bwd_q4_kernel<T, false, DET>, Q4Smem<T, false>::TOTAL);
 }
 
 }  // namespace zg

@@ -22,6 +22,39 @@ void zg_note_scan_kernel(const char *name);      // which forward-scan kernel th
 
 static inline int zg_dtype_size(int dt) { return dt == ZG_F32 ? 4 : 2; }
 
+// ---- deterministic backward (the *_bwd_det entry points) ---------------------------------------
+// The DET instantiation of a backward kernel stores each value it would have added with an fp32 atomic into its own row
+// of a partials region: rows x n floats, the row fixed by the static grid mapping (tile, batch row, chunk index).
+// zg_reduce_rows then adds the rows into the zero-filled output in row order, so the result does not depend on the
+// order in which CTAs ran.  ZgDetLayout carves one region per reduced output out of the caller's workspace; the same
+// code sizes the workspace (ws == nullptr) and hands out the region pointers, so the size query and the launch agree.
+int zg_reduce_rows(const float *part, int64_t rows, int64_t n, float *out, cudaStream_t s);
+
+struct ZgDetLayout {
+    struct Region { float *out, *part; int64_t rows, n; };
+    Region reg[8];
+    int count = 0;
+    int64_t bytes = 0;
+    unsigned char *ws = nullptr;
+    // region of rows x n floats for `out` (nothing when out is NULL); returns where the kernel writes its partials
+    float *add(float *out, int64_t rows, int64_t n) {
+        if (out == nullptr || rows <= 0 || n <= 0) return nullptr;
+        float *part = ws ? reinterpret_cast<float *>(ws + bytes) : nullptr;
+        reg[count++] = Region{out, part, rows, n};
+        bytes += (rows * n * (int64_t)sizeof(float) + 15) / 16 * 16;
+        return part;
+    }
+    int reduce(cudaStream_t s) const {
+        for (int i = 0; i < count; ++i)
+            if (int rc = zg_reduce_rows(reg[i].part, reg[i].rows, reg[i].n, reg[i].out, s)) return rc;
+        return 0;
+    }
+};
+// checks the caller's workspace against the layout (which must have been built with ws set)
+#define ZG_REQUIRE_WORKSPACE(lay, ws, ws_bytes, who)                                                                  \
+    ZG_REQUIRE((lay).bytes <= (ws_bytes) && ((lay).bytes == 0 || ((ws) != nullptr && (reinterpret_cast<uintptr_t>(ws) & 15) == 0)), \
+               "%s: workspace of %lld bytes (16-byte aligned) needed, got %lld", who, (long long)(lay).bytes, (long long)(ws_bytes))
+
 // ---- device helpers ---------------------------------------------------------------------------
 #define ZG_LOG2E 1.4426950408889634f
 #define ZG_LN2 0.6931471805599453f

@@ -53,7 +53,7 @@ def _norm_bwd(dy, x, weight, bias, mean, rstd, dresidual, has_residual, is_rms, 
     if dy.dtype != x_dtype:
         dy = dy.to(x_dtype)
         p.dy, p.dy_rs = _lib.ptr(dy), dy.stride(0)
-    _lib.call("zg_add_norm_bwd", p)
+    _lib.call_bwd("zg_add_norm_bwd", p)
     if has_residual and dx.dtype == x.dtype:
         dres_in = dx
     return dx, (dw.to(weight.dtype) if dw is not None else None), (db.to(bias.dtype) if db is not None else None), dres_in

@@ -222,7 +222,7 @@ def _scan_bwd(saved, ckpt, dout, delta_softplus, dz_out=None, z_rowmap=None):
     if dz is not None:
         q.dz_sb, q.dz_sd, q.dz_sl = _strides3(dz)
     q.dA, q.dD, q.ddelta_bias, q.dB, q.dC = _lib.ptr(dA), _lib.ptr(dD), _lib.ptr(dbias), _lib.ptr(dB), _lib.ptr(dC)
-    _lib.call("zg_selective_scan_bwd", q)
+    _lib.call_bwd("zg_selective_scan_bwd", q)
     return du, ddelta, dA, dB, dC, dD, dbias, dz
 
 
