@@ -212,6 +212,8 @@ int zg_add_norm_bwd(const zg_norm_bwd_params *p, void *stream);
  *     normed   = r * rsqrt(mean(r^2) + eps) * norm_w            (dtype; the next block's x)
  *     modded   = normed * (1 + scale[b,:]) + shift[b,:]         (dtype; the next in_proj input)
  * gate/shift/scale are (batch, dim) with row stride mod_rs (views into adaLN's (batch, 3*dim)).
+ * Alignment (here and in the backward): row tensors 16 bytes; gate/shift/scale/norm_w 4 elements (8 bytes for 16-bit
+ * dtypes, 16 for fp32) with mod_rs % 4 == 0.
  * With final != 0 the last two lines become the model tail (model_zigma.py:971-984,335):
  *     normed = LayerNorm_noaffine(normed, eps=1e-6) and modded is not written.
  * Intermediate roundings replicate the reference's unfused bf16 path: hidden and normed are

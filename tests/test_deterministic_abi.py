@@ -176,6 +176,76 @@ def test_det_call_rejects_small_workspace():
     assert rc != 0 and b"nparts" in l.zg_last_error()
 
 
+def test_tail_bwd_nparts_gives_every_batch_element_a_warp():
+    """block_ops.tail_bwd_nparts, the CTA count of both block-tail backward kernels: at least one warp per batch element
+    (small seqlen with a large batch, or a batch past 4 x 3 CTAs per SM), never more CTAs than the kernel accepts, and a
+    batch beyond that a clear error rather than a failed launch."""
+    from zigma_b200.block_ops import tail_bwd_nparts
+    for sms in (1, 78, 114, 132, 148):
+        for B in (1, 2, 3, 4, 5, 8, 9, 16, 64, 1584, 1585, 1600, 4096, 65535, 262140):
+            for L in (1, 4, 5, 15, 16, 37, 256, 1024, 4096):
+                n = tail_bwd_nparts(B, L, sms)
+                assert 1 <= n <= 65535 and 4 * n >= B, (B, L, sms, n)
+                assert n == max(1, min((B * L + 63) // 64, 3 * sms), (B + 3) // 4)
+    assert tail_bwd_nparts(8, 4, 132) == 2 and tail_bwd_nparts(16, 1024, 132) == 256
+    with pytest.raises(RuntimeError, match="65535"):
+        tail_bwd_nparts(262141, 1, 132)
+
+
+def _tail_fwd_params(_lib, dtype, dim, gate_off=0, scale_off=0):
+    """Forward params of an EMPTY batch whose modulation vectors are views of one (batch, 3 dim) buffer at fake addresses: the
+    argument checks run before the empty-batch return, so no kernel can be launched whatever they decide."""
+    esz = 4 if dtype == _lib.ZG_F32 else 2
+    p = _lib.BlockTailParams()
+    _ptrs(p, ["x", "mix", "norm_w", "residual", "residual_out", "normed", "modded"])
+    base = FAKE * 64
+    p.gate, p.shift, p.scale = base + gate_off, base + dim * esz, base + 2 * dim * esz + scale_off
+    p.mod_rs = 3 * dim
+    p.batch, p.seqlen, p.dim, p.dtype = 0, 16, dim, dtype
+    return p
+
+
+def test_tail_modulation_alignment_checks():
+    """zg_block_tail_fwd / _fwd_pe / _bwd read gate / shift / scale / norm_w as 4-element vectors: a pointer 2 bytes off is
+    rejected by all three, while the views of a (batch, 3 dim) 16-bit buffer at dim = 36 (scale 144 bytes in, 8-byte
+    aligned only) are accepted, forward and backward."""
+    _lib = _built()
+    l = _lib.lib()
+
+    def fwd(name, p):
+        if name == "zg_block_tail_fwd_pe":
+            p.gate = p.residual = None
+        return getattr(l, name)(C.byref(p), C.c_void_p(None))
+
+    def bwd(p):
+        q = _lib.BlockTailBwdParams()
+        _ptrs(q, ["d_residual_out", "d_normed", "d_modded", "r", "rstd", "mix", "d_x", "d_mix", "d_residual_in",
+                  "dgate", "dshift", "dscale", "d_norm_w"])
+        q.gate, q.scale, q.norm_w = p.gate, p.scale, p.norm_w
+        q.mod_rs, q.batch, q.seqlen, q.dim, q.dtype, q.nparts = p.mod_rs, 0, p.seqlen, p.dim, p.dtype, 1
+        return l.zg_block_tail_bwd(C.byref(q), C.c_void_p(None))
+
+    for dt in (_lib.ZG_F32, _lib.ZG_F16, _lib.ZG_BF16):
+        for dim in (36, 100, 640):
+            for name in ("zg_block_tail_fwd", "zg_block_tail_fwd_pe"):
+                assert fwd(name, _tail_fwd_params(_lib, dt, dim)) == 0, (name, dt, dim, l.zg_last_error())
+            assert bwd(_tail_fwd_params(_lib, dt, dim)) == 0, (dt, dim, l.zg_last_error())
+            for off in ("gate_off", "scale_off"):
+                p = _tail_fwd_params(_lib, dt, dim, **{off: 2})
+                for name in ("zg_block_tail_fwd", "zg_block_tail_fwd_pe"):
+                    if name == "zg_block_tail_fwd_pe" and off == "gate_off":
+                        continue                   # the positional-embedding tail takes no gate
+                    assert fwd(name, _tail_fwd_params(_lib, dt, dim, **{off: 2})) != 0, (name, off, dt, dim)
+                    assert b"aligned" in l.zg_last_error()
+                assert bwd(p) != 0 and b"aligned" in l.zg_last_error(), (off, dt, dim)
+        p = _tail_fwd_params(_lib, dt, 64)
+        p.norm_w += 2
+        assert fwd("zg_block_tail_fwd", p) != 0 and bwd(p) != 0 and b"aligned" in l.zg_last_error()
+    # fp32 needs 16 bytes: 8 bytes off, enough for a 16-bit vector, is rejected
+    p = _tail_fwd_params(_lib, _lib.ZG_F32, 36, scale_off=8)
+    assert fwd("zg_block_tail_fwd", p) != 0 and bwd(p) != 0
+
+
 # kernel families with a DET instantiation (DET is the last template argument of each)
 DET_KERNELS = ["scan_bwd_q4_kernel", "scan_bwd_kernel", "conv_bwd_seqc_kernel", "conv_bwd_seqc_vec_kernel", "conv_bwd_tok_kernel",
                "conv_bwd_tok4_kernel", "add_norm_bwd_kernel", "add_norm_bwd_vec_kernel", "block_tail_bwd_kernel"]

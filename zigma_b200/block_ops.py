@@ -20,6 +20,16 @@ def _contig(t):
     return None if t is None else (t if t.is_contiguous() else t.contiguous())
 
 
+def tail_bwd_nparts(batch, seqlen, sms):
+    """CTAs of zg_block_tail_bwd, which are also the rows of its d_norm_w partials buffer: about one per 64 token rows, at
+    most 3 per SM, and at least one warp (4 per CTA) per batch element, which the deterministic kernel needs.  The atomic
+    and the deterministic kernel get the same value, so their d_norm_w partial rows have the same layout."""
+    nparts = max(1, min((batch * seqlen + 63) // 64, 3 * sms), (batch + 3) // 4)
+    if nparts > 65535:
+        raise RuntimeError(f"block_tail_fn backward: batch {batch} needs {nparts} CTAs, more than the 65535 the kernel takes")
+    return nparts
+
+
 class BlockTailFn(torch.autograd.Function):
     """(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps) -> (residual_out fp32, normed, modded).
     x, mix: (B, L, D) contiguous; gate / shift / scale: (B, D) views with one common row stride (chunks of adaLN's
@@ -52,7 +62,7 @@ class BlockTailFn(torch.autograd.Function):
         d_mix = torch.empty((B, L, D), dtype=act, device=dev) if mix is not None else None
         d_res_in = torch.empty((B, L, D), dtype=torch.float32, device=dev) if ctx.has_res else None
         acc = torch.zeros((3, B, D), dtype=torch.float32, device=dev)
-        nparts = max(1, min((B * L + 63) // 64, 3 * torch.cuda.get_device_properties(dev).multi_processor_count))
+        nparts = tail_bwd_nparts(B, L, torch.cuda.get_device_properties(dev).multi_processor_count)
         d_w = torch.empty((nparts, D), dtype=torch.float32, device=dev)       # per-CTA partial sums, added up below
         nw = norm_w if norm_w.dtype == act else norm_w.to(act)
         q = _lib.BlockTailBwdParams()

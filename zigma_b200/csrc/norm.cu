@@ -842,6 +842,10 @@ template <typename T, bool DET> static int norm_bwd_t(const zg_norm_bwd_params &
 }  // namespace zg
 
 static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+// the block tail reads gate / shift / scale / norm_w as 4-element vectors (ld4 / ldraw): 8 bytes for 16-bit dtypes, 16 for fp32
+static bool aligned_quad(const void *p, int dtype) {
+    return (reinterpret_cast<uintptr_t>(p) & (4 * (dtype == ZG_F32 ? sizeof(float) : sizeof(__half)) - 1)) == 0;
+}
 
 extern "C" int zg_add_norm_fwd(const zg_norm_params *pp, void *stream) {
     ZG_REQUIRE(pp != nullptr, "add_norm_fwd: null params");
@@ -925,6 +929,8 @@ static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bo
     ZG_REQUIRE(p.mod_rs % 4 == 0, "block_tail_fwd: modulation row stride must be a multiple of 4");
     ZG_REQUIRE(aligned16(p.x) && aligned16(p.mix) && aligned16(p.residual) && aligned16(p.residual_out) && aligned16(p.normed) && aligned16(p.modded),
                "block_tail_fwd: row tensors must be 16-byte aligned");
+    ZG_REQUIRE(aligned_quad(p.gate, p.dtype) && aligned_quad(p.shift, p.dtype) && aligned_quad(p.scale, p.dtype) && aligned_quad(p.norm_w, p.dtype),
+               "block_tail_fwd: gate / shift / scale / norm_w must be aligned to 4 elements");
     const int64_t nrows = (int64_t)p.batch * p.seqlen;
     if (nrows == 0) return 0;
     cudaStream_t s = (cudaStream_t)stream;
@@ -946,10 +952,12 @@ static int block_tail_bwd_validate(const zg_block_tail_bwd_params &p) {
     ZG_REQUIRE(p.dim > 0 && p.dim % 4 == 0 && p.dim <= 1024, "block_tail_bwd: dim must be a multiple of 4 and <= 1024, got %d", p.dim);
     ZG_REQUIRE(p.mod_rs % 4 == 0, "block_tail_bwd: modulation row stride must be a multiple of 4");
     ZG_REQUIRE(p.nparts >= 1 && p.nparts <= 65535, "block_tail_bwd: nparts (rows of the d_norm_w partials buffer = CTAs) must be in [1, 65535]");
-    ZG_REQUIRE(aligned16(p.r) && aligned16(p.d_residual_out) && aligned16(p.d_normed) && aligned16(p.d_modded) && aligned16(p.mix) && aligned16(p.d_x) &&
-                   aligned16(p.d_mix) && aligned16(p.d_residual_in) && aligned16(p.gate) && aligned16(p.scale) && aligned16(p.norm_w),
-               "block_tail_bwd: tensors must be 16-byte aligned");
     ZG_REQUIRE(p.dtype == ZG_F32 || p.dtype == ZG_F16 || p.dtype == ZG_BF16, "block_tail_bwd: bad dtype %d", p.dtype);
+    ZG_REQUIRE(aligned16(p.r) && aligned16(p.d_residual_out) && aligned16(p.d_normed) && aligned16(p.d_modded) && aligned16(p.mix) && aligned16(p.d_x) &&
+                   aligned16(p.d_mix) && aligned16(p.d_residual_in),
+               "block_tail_bwd: row tensors must be 16-byte aligned");
+    ZG_REQUIRE(aligned_quad(p.gate, p.dtype) && aligned_quad(p.scale, p.dtype) && aligned_quad(p.norm_w, p.dtype),
+               "block_tail_bwd: gate / scale / norm_w must be aligned to 4 elements");
     return 0;
 }
 
