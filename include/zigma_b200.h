@@ -295,6 +295,53 @@ int64_t zg_block_tail_bwd_det_workspace_bytes(const zg_block_tail_bwd_params *p)
 int zg_block_tail_bwd_det(const zg_block_tail_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Text cross-attention of has_text blocks (model_zigma.py:95-135; DESIGN.md section 4.7), per (batch, head):
+ *     O = softmax(Q K^T * 0.125) V          head dimension 64, no mask, no dropout
+ * Q, O (batch, L, dim) and K, V (batch, Lk, dim) token-major, dim = heads * 64, head h in columns [64 h, 64 h + 64) of
+ * every row; columns contiguous, rows and batches at the given strides (elements).  1 <= Lk <= 256; any heads >= 1;
+ * dtype fp32, fp16 or bf16 for all four.  lse (batch, heads, L) fp32 contiguous, or NULL: the natural-log log-sum-exp
+ * log(sum_j exp(0.125 q.k_j)) of each row, written by the forward, read by the backward.
+ * Alignment: q, k, v, o (and dout, dq, dk, dv of the backward) 16-byte aligned, with batch and row strides whole multiples
+ * of 16 bytes (8 elements for 16-bit dtypes, 4 for fp32): column slices of a fused (rows, 3 dim) buffer qualify.
+ * Errors (nothing launched): Lk outside [1, 256], dim not a multiple of 64 or != 64 heads, a misaligned pointer or stride,
+ * a workspace too small.  batch == 0 or L == 0 passes the checks and launches nothing.
+ * Roundings: 16-bit -- S = Q K^T and O = P V accumulate in fp32 on the tensor cores, P is rounded to the I/O dtype as the
+ * A operand of P V, O divided by the fp32 row sum once and rounded once at the store; fp32 -- CUDA cores, same formula.
+ */
+typedef struct {
+    const void *q, *k, *v;
+    void *o;
+    float *lse;
+    int64_t q_sb, q_rs, k_sb, k_rs, v_sb, v_rs, o_sb, o_rs;
+    int32_t batch, L, Lk, heads, dim, dtype;
+} zg_xattn_params;
+
+int zg_cross_attn_fwd(const zg_xattn_params *p, void *stream);
+
+/* Backward: inputs dout (like o), fwd.q / k / v, fwd.o (the forward's output) and fwd.lse; outputs dq (like q), dk, dv
+ * (like k, v), all written (no zero-fill needed).  P is recomputed from lse, D_i = sum dout_i o_i, dS = P (dout V^T - D),
+ * dq = 0.125 dS K, dk = 0.125 dS^T Q, dv = P^T dout, in fp32, rounded once at the store.  No floating-point atomics: the
+ * dk / dv sums over the L query rows are taken per segment of whole 64-row query tiles into the workspace, then added in
+ * segment order, so the result is bitwise reproducible whatever the CTA order (and whatever torch's deterministic flag).
+ * sms (>= 1) is the SM count of the device; it fixes the segment count:
+ *     tiles = ceil(L / 64),  ctas = batch * heads * ceil(Lk / 32),  n = min(tiles, ceil(8 sms / ctas)),
+ *     per = ceil(tiles / n),  nseg = ceil(tiles / per)          (segments of per * 64 query rows)
+ * workspace: at least zg_cross_attn_bwd_workspace_bytes(p) bytes, 16-byte aligned, no initial contents needed:
+ *     roundup16(4 batch heads L) + 2 * 4 * nseg * batch * heads * Lk * 64        (0 when batch, L or heads is 0)
+ * (D per row, then the fp32 dk and dv partials per segment).  Equal bits across devices need equal sms.
+ * zg_cross_attn_bwd_workspace_bytes is host arithmetic only.  batch * heads <= 65535. */
+typedef struct {
+    zg_xattn_params fwd;
+    const void *dout;
+    void *dq, *dk, *dv;
+    int64_t dout_sb, dout_rs, dq_sb, dq_rs, dk_sb, dk_rs, dv_sb, dv_rs;
+    int32_t sms;
+} zg_xattn_bwd_params;
+
+int64_t zg_cross_attn_bwd_workspace_bytes(const zg_xattn_bwd_params *p);
+int zg_cross_attn_bwd(const zg_xattn_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * bf16 GEMM on the Hopper tensor cores (wgmma):  C[M,N] = A[M,K] * B[N,K]^T (+ bias[N]), fp32 accumulate in
  * registers, bf16 output.  A, B row-major with leading dims lda/ldb (elements, multiples of 8);
  * C row-major ldc.  out_rowmap (int32[rows_per_batch] or NULL): output row m of batch

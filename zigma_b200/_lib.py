@@ -78,6 +78,19 @@ class BlockTailBwdParams(C.Structure):
                 + [(n, i32) for n in ("batch", "seqlen", "dim", "dtype", "nparts")])
 
 
+class XattnParams(C.Structure):
+    _fields_ = ([(n, vp) for n in ("q", "k", "v", "o", "lse")]
+                + [(n, i64) for n in ("q_sb", "q_rs", "k_sb", "k_rs", "v_sb", "v_rs", "o_sb", "o_rs")]
+                + [(n, i32) for n in ("batch", "L", "Lk", "heads", "dim", "dtype")])
+
+
+class XattnBwdParams(C.Structure):
+    _fields_ = ([("fwd", XattnParams)]
+                + [(n, vp) for n in ("dout", "dq", "dk", "dv")]
+                + [(n, i64) for n in ("dout_sb", "dout_rs", "dq_sb", "dq_rs", "dk_sb", "dk_rs", "dv_sb", "dv_rs")]
+                + [("sms", i32)])
+
+
 class GemmParams(C.Structure):
     _fields_ = ([(n, vp) for n in ("A", "B", "bias", "C", "out_rowmap")]
                 + [(n, i64) for n in ("lda", "ldb", "ldc")]
@@ -97,6 +110,8 @@ EXPORTS = ["zg_abi_version", "zg_last_error", "zg_launch_count", "zg_last_scan_k
 # deterministic backward twins (zg_<op>_det + zg_<op>_det_workspace_bytes) of these entry points
 DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd"]
 EXPORTS += [n + s for n in DET_OPS for s in ("_det", "_det_workspace_bytes")]
+# cross-attention (always atomic-free, so no _det twin); the last two have signatures of their own
+EXPORTS += ["zg_cross_attn_fwd", "zg_cross_attn_bwd", "zg_cross_attn_bwd_workspace_bytes"]
 
 _lib = None
 
@@ -126,6 +141,9 @@ def lib():
             else:
                 getattr(l, name).restype = C.c_int
                 getattr(l, name).argtypes = [C.c_void_p, C.c_void_p]
+        l.zg_cross_attn_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+        l.zg_cross_attn_bwd_workspace_bytes.restype = C.c_int64
+        l.zg_cross_attn_bwd_workspace_bytes.argtypes = [C.c_void_p]
         _lib = l
     return _lib
 

@@ -340,7 +340,7 @@ class ZigMaEngine:
             scale = None if last else mods[:, i + 1, 1]
             if m.has_text:
                 # text blocks (model_zigma.py:446-458): the mixer's gated residual has to exist before the cross-attention
-                # reads it; the attention branch (library SDPA on 77 text tokens) then takes the place of the mixer output
+                # reads it; the attention branch (zg_cross_attn_fwd on the text tokens) then takes the place of the mixer output
                 # in the fused tail:  hidden2 = hidden + gate_msa * msa(modulate(norm_msa(hidden)))
                 blk = m.blocks[i]
                 # un-permute the mixer output with the layer's own row table: (B fold, L / fold) rows for a spatial video layer

@@ -14,6 +14,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from .attention import MAX_KEYS, cross_attention_fn
 from .layernorm import RMSNorm, layer_norm_fn, rms_norm_fn
 from .mamba_simple import Mamba
 from .utils_zigzag import hilbert_path, reverse_permut_np, zigzag_path
@@ -62,8 +63,9 @@ class PatchEmbed_Video(PatchEmbed):
 
 
 class CrossAttention(nn.Module):
-    """Text cross-attention of has_text blocks (model_zigma.py:95-135); library SDPA, not on the
-    benchmarked path (none of the BASELINE configs sets has_text)."""
+    """Text cross-attention of has_text blocks (model_zigma.py:95-135).  CUDA tensors with 1 <= Lk <= 256 text tokens run
+    on zg_cross_attn_fwd / _bwd (attention.py), reading and writing the token-major projections directly; CPU tensors and
+    longer contexts use library SDPA."""
 
     def __init__(self, query_dim, context_dim=None, heads=8, dim_head=64, dropout=0.0):
         super().__init__()
@@ -76,9 +78,12 @@ class CrossAttention(nn.Module):
         self.to_out = nn.Sequential(nn.Linear(inner, query_dim), nn.Dropout(dropout))
 
     def forward(self, x, text, mask=None):
+        q, k, v = self.to_q(x), self.to_k(text), self.to_v(text)
+        if q.is_cuda and 1 <= k.shape[1] <= MAX_KEYS:
+            return self.to_out(cross_attention_fn(q, k, v, self.heads))
         B = x.shape[0]
         split = lambda t: t.reshape(B, t.shape[1], self.heads, -1).transpose(1, 2)
-        o = F.scaled_dot_product_attention(split(self.to_q(x)), split(self.to_k(text)), split(self.to_v(text)))
+        o = F.scaled_dot_product_attention(split(q), split(k), split(v))
         return self.to_out(o.transpose(1, 2).reshape(B, x.shape[1], -1))
 
 
