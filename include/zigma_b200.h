@@ -295,6 +295,40 @@ int64_t zg_block_tail_bwd_det_workspace_bytes(const zg_block_tail_bwd_params *p)
 int zg_block_tail_bwd_det(const zg_block_tail_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Block tail with stochastic depth (training with drop_path_rate > 0; model_zigma.py:138-160,416-438).  The reference's
+ * Block applies its DropPath to the previous block's hidden before the fused add+norm: with s[b] the multiplier it drew
+ * for batch element b (0 or round_to_dtype(1 / keep), a tensor value, never recomputed here):
+ *     hidden   = round(x + round(gate * mix[rowmap]))           (as zg_block_tail_fwd)
+ *     kept     = round(hidden * s[b])                           (new: the eager `x * mask`, rounded before the add)
+ *     r        = residual + kept            (fp32, residual_out)
+ *     normed, modded, rstd                                      (as zg_block_tail_fwd)
+ * and in the backward, with dr = rmsnorm_bwd(...) + d_residual_out as in zg_block_tail_bwd:
+ *     d_residual_in = dr                                        (the multiplier is not on the residual path)
+ *     dh = round(round(dr) * s[b]);   d_x = dh;   d_mix[rowmap[l]] = round(gate * dh[l]);   dgate[b] += sum_l dh[l] * mix[rowmap[l]]
+ *     dshift, dscale, d_norm_w                                  (as zg_block_tail_bwd: they do not see the multiplier)
+ * With s == 1 the results equal the plain entry points' bit for bit; with s[b] == 0 the d_x, d_mix rows and the dgate row
+ * of b are zero.
+ *   path_scale: (batch) in `dtype`, aligned to its element size, read once per token row.
+ * Everything the plain entry points take and check applies, plus: path_scale, residual (forward) and mix non-NULL (the first
+ * block has no residual and so no drop path), final_layer == 0 and dim <= 1024.  The forward runs the four-warps-per-row
+ * kernel; the backward has the plain one's grid, nparts contract and, for the _det twin, the same workspace
+ * (zg_block_tail_bwd_dp_det_workspace_bytes returns what zg_block_tail_bwd_det_workspace_bytes returns for `base`). */
+typedef struct {
+    zg_block_tail_params base;
+    const void *path_scale;
+} zg_block_tail_dp_params;
+
+typedef struct {
+    zg_block_tail_bwd_params base;
+    const void *path_scale;
+} zg_block_tail_bwd_dp_params;
+
+int zg_block_tail_fwd_dp(const zg_block_tail_dp_params *p, void *stream);
+int zg_block_tail_bwd_dp(const zg_block_tail_bwd_dp_params *p, void *stream);
+int64_t zg_block_tail_bwd_dp_det_workspace_bytes(const zg_block_tail_bwd_dp_params *p);
+int zg_block_tail_bwd_dp_det(const zg_block_tail_bwd_dp_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Text cross-attention of has_text blocks (model_zigma.py:95-135; DESIGN.md section 4.7), per (batch, head):
  *     O = softmax(Q K^T * 0.125) V          head dimension 64, no mask, no dropout
  * Q, O (batch, L, dim) and K, V (batch, Lk, dim) token-major, dim = heads * 64, head h in columns [64 h, 64 h + 64) of

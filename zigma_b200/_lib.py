@@ -78,6 +78,14 @@ class BlockTailBwdParams(C.Structure):
                 + [(n, i32) for n in ("batch", "seqlen", "dim", "dtype", "nparts")])
 
 
+class BlockTailDpParams(C.Structure):
+    _fields_ = [("base", BlockTailParams), ("path_scale", vp)]
+
+
+class BlockTailBwdDpParams(C.Structure):
+    _fields_ = [("base", BlockTailBwdParams), ("path_scale", vp)]
+
+
 class XattnParams(C.Structure):
     _fields_ = ([(n, vp) for n in ("q", "k", "v", "o", "lse")]
                 + [(n, i64) for n in ("q_sb", "q_rs", "k_sb", "k_rs", "v_sb", "v_rs", "o_sb", "o_rs")]
@@ -106,9 +114,10 @@ class AdamWParams(C.Structure):
 
 EXPORTS = ["zg_abi_version", "zg_last_error", "zg_launch_count", "zg_last_scan_kernel", "zg_scan_kernel_choice", "zg_selective_scan_fwd", "zg_selective_scan_bwd",
            "zg_causal_conv1d_fwd", "zg_causal_conv1d_bwd", "zg_add_norm_fwd", "zg_add_norm_bwd",
-           "zg_block_tail_fwd", "zg_block_tail_fwd_pe", "zg_block_tail_bwd", "zg_gemm_bf16_tn", "zg_adamw_ema_step"]
+           "zg_block_tail_fwd", "zg_block_tail_fwd_pe", "zg_block_tail_bwd", "zg_block_tail_fwd_dp", "zg_block_tail_bwd_dp",
+           "zg_gemm_bf16_tn", "zg_adamw_ema_step"]
 # deterministic backward twins (zg_<op>_det + zg_<op>_det_workspace_bytes) of these entry points
-DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd"]
+DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd", "zg_block_tail_bwd_dp"]
 EXPORTS += [n + s for n in DET_OPS for s in ("_det", "_det_workspace_bytes")]
 # cross-attention (always atomic-free, so no _det twin); the last two have signatures of their own
 EXPORTS += ["zg_cross_attn_fwd", "zg_cross_attn_bwd", "zg_cross_attn_bwd_workspace_bytes"]

@@ -31,12 +31,14 @@ def tail_bwd_nparts(batch, seqlen, sms):
 
 
 class BlockTailFn(torch.autograd.Function):
-    """(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps) -> (residual_out fp32, normed, modded).
+    """(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, path_scale) -> (residual_out fp32, normed, modded).
     x, mix: (B, L, D) contiguous; gate / shift / scale: (B, D) views with one common row stride (chunks of adaLN's
-    (B, 3D) output); residual: (B, L, D) fp32 or None; rowmap: int32 (L,) or None; mix / gate None for the first block."""
+    (B, 3D) output); residual: (B, L, D) fp32 or None; rowmap: int32 (L,) or None; mix / gate None for the first block.
+    path_scale: None, or the block's drop-path multipliers (B,) in x.dtype (stochastic depth in training): the hidden
+    state joins the residual as hidden * path_scale[b] (zg_block_tail_fwd_dp / _bwd_dp); it gets no gradient."""
 
     @staticmethod
-    def forward(ctx, x, mix, gate, shift, scale, norm_w, residual, rowmap, eps):
+    def forward(ctx, x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, path_scale=None):
         x, mix, residual = _contig(x), _contig(mix), _contig(residual)
         # one dtype for every operand of the kernels (x's): see engine.block_tail.  The casts happen HERE so that the
         # tensors saved for the backward are the ones the forward kernel actually read.
@@ -46,14 +48,15 @@ class BlockTailFn(torch.autograd.Function):
         mods = [m for m in (gate, shift, scale) if m is not None]
         if mods and any(m.stride(0) != mods[0].stride(0) or m.stride(1) != 1 for m in mods):
             gate, shift, scale = [None if m is None else m.contiguous() for m in (gate, shift, scale)]
-        res_out, normed, modded, rstd = block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, want_rstd=True)
-        ctx.save_for_backward(res_out, rstd, mix, gate, scale, norm_w, rowmap)
+        res_out, normed, modded, rstd = block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, want_rstd=True,
+                                                   path_scale=path_scale)
+        ctx.save_for_backward(res_out, rstd, mix, gate, scale, norm_w, rowmap, path_scale)
         ctx.has_res = residual is not None
         return res_out, normed, modded
 
     @staticmethod
     def backward(ctx, d_res_out, d_normed, d_modded):
-        res_out, rstd, mix, gate, scale, norm_w, rowmap = ctx.saved_tensors
+        res_out, rstd, mix, gate, scale, norm_w, rowmap, path_scale = ctx.saved_tensors
         B, L, D = res_out.shape
         act = scale.dtype
         dev = res_out.device
@@ -73,11 +76,14 @@ class BlockTailFn(torch.autograd.Function):
         q.dgate, q.dshift, q.dscale, q.d_norm_w = (_lib.ptr(acc[0]) if mix is not None else None), _lib.ptr(acc[1]), _lib.ptr(acc[2]), _lib.ptr(d_w)
         q.mod_rs = scale.stride(0)
         q.batch, q.seqlen, q.dim, q.dtype, q.nparts = B, L, D, _lib.dt(act), nparts
-        _lib.call_bwd("zg_block_tail_bwd", q)
+        if path_scale is None:
+            _lib.call_bwd("zg_block_tail_bwd", q)
+        else:
+            _lib.call_bwd("zg_block_tail_bwd_dp", _lib.BlockTailBwdDpParams(q, _lib.ptr(path_scale)))
         dt_mix, dt_gate, dt_shift, dt_scale = ctx.in_dtypes
         return (d_x, None if d_mix is None else d_mix.to(dt_mix), acc[0].to(dt_gate) if mix is not None else None,
-                acc[1].to(dt_shift or act), acc[2].to(dt_scale or act), d_w.sum(0).to(norm_w.dtype), d_res_in, None, None)
+                acc[1].to(dt_shift or act), acc[2].to(dt_scale or act), d_w.sum(0).to(norm_w.dtype), d_res_in, None, None, None)
 
 
-def block_tail_fn(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps):
-    return BlockTailFn.apply(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps)
+def block_tail_fn(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, path_scale=None):
+    return BlockTailFn.apply(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, path_scale)

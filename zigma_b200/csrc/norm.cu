@@ -444,8 +444,10 @@ __global__ void __launch_bounds__(128, (MAXQ <= 6) ? 6 : 1) block_tail_kernel(co
 // PE (zg_block_tail_fwd_pe, the first tail of a forward): mix is the (seqlen, dim) positional-embedding table shared by every
 // batch element and there is no gate: hidden = round(tokens + pos_embed), the reference's `x = x + self.pos_embed`
 // (model_zigma.py:941), without an elementwise pass of its own.  A separate instantiation: the per-layer instance is unchanged.
-template <typename T, int MAXQ, bool PE>
-__global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(const zg_block_tail_params p) {
+// DP (zg_block_tail_fwd_dp, stochastic depth in training): hidden is multiplied by the batch element's drop-path multiplier
+// before the residual add, kept = round(hidden * path_scale[b]), the reference's eager `x * mask`.  One scalar load per row.
+template <typename T, int MAXQ, bool PE, bool DP>
+__device__ __forceinline__ void block_tail_row4_body(const zg_block_tail_params &p, const void *path_scale) {
     __shared__ float red[3][4];
     const int64_t row = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -491,6 +493,8 @@ __global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(cons
 #endif
         }
     }
+    float dps = 1.f;
+    if constexpr (DP) dps = zg_to_float<T>(reinterpret_cast<const T *>(path_scale)[b]);
     float r[MAXQ][4];
     float sumsq = 0.f;
 #pragma unroll
@@ -505,6 +509,10 @@ __global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(cons
 #pragma unroll
                 for (int i = 0; i < 4; ++i)   // x + gate * mixer(...)  each op rounded to T as in eager torch
                     r[k][i] = round_to<T>(r[k][i] + round_to<T>(g[i] * m[i]));
+            }
+            if constexpr (DP) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) r[k][i] = round_to<T>(__fmul_rn(r[k][i], dps));   // rounded before the add (no FMA)
             }
             if (res) {
                 r[k][0] += rr[k].x; r[k][1] += rr[k].y; r[k][2] += rr[k].z; r[k][3] += rr[k].w;
@@ -530,7 +538,7 @@ __global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(cons
             }
         }
     }
-    if (p.final_layer) {
+    if (!DP && p.final_layer) {      // (the drop-path entry point rejects final_layer)
         // norm_final = LayerNorm(no affine, eps 1e-6) on the materialised norm_f output (model_zigma.py:320,335)
         const float mean = block_sum(sum2, 1) / D;
         float s2 = 0.f;
@@ -575,6 +583,25 @@ __global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(cons
     }
 }
 
+template <typename T, int MAXQ, bool PE>
+__global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(const zg_block_tail_params p) {
+    block_tail_row4_body<T, MAXQ, PE, false>(p, nullptr);
+}
+
+template <typename T, int MAXQ>
+__global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_dp_fwd_kernel(const zg_block_tail_dp_params p) {
+    block_tail_row4_body<T, MAXQ, false, true>(p.base, p.path_scale);
+}
+
+// zg_block_tail_fwd_dp: the four-warps-per-row kernel only (dim <= 1024 -> Q 1 or 2, checked by the entry point)
+template <typename T> static int block_tail_dp_t(const zg_block_tail_dp_params &p, cudaStream_t s) {
+    const unsigned g4 = (unsigned)((int64_t)p.base.batch * p.base.seqlen);
+    if (p.base.dim <= 512) block_tail_dp_fwd_kernel<T, 1><<<g4, 128, 0, s>>>(p);
+    else block_tail_dp_fwd_kernel<T, 2><<<g4, 128, 0, s>>>(p);
+    zg_count_launch();
+    return zg_check_launch("block_tail_fwd_dp");
+}
+
 template <typename T> static int block_tail_t(const zg_block_tail_params &p, cudaStream_t s, bool pe = false) {
     const int64_t nrows = (int64_t)p.batch * p.seqlen;
     static int row4 = -1;       // ZG_TAIL_ROW4=0: the round-1 kernel (one warp per row)
@@ -616,182 +643,39 @@ constexpr int TAILB_ROWS = 16;
 // contiguous share of the rows of element w / wpb (warps past batch * wpb idle) -- so that a warp never crosses a batch
 // boundary; dgate / dshift / dscale of p address partial rows, one per warp index within the element, (wpb, batch, dim),
 // stored (zeros for a warp without rows), not added (zg_block_tail_bwd_det).  d_norm_w is the same partials buffer in both.
+// DP (zg_block_tail_bwd_dp): the gradient reaching hidden through the forward's `hidden * path_scale[b]` is
+// dh = round(round(dr) * path_scale[b]); d_x, d_mix and dgate follow from that dh, everything else is unchanged.
 template <typename T, int MAXQ, bool DET>
 __global__ void __launch_bounds__(128, 3) block_tail_bwd_kernel(const zg_block_tail_bwd_params p) {
-    // per-batch column sums live in shared memory (lane-private slots, no conflicts): keeping all four accumulator sets
-    // in registers cost 212 registers = 8 warps per SM, too few for a streaming kernel
-    extern __shared__ __align__(16) float tailb_smem[];
-    float4 *acc_s = reinterpret_cast<float4 *>(tailb_smem) + (threadIdx.x >> 5) * (3 * MAXQ * 32) + (threadIdx.x & 31);   // [warp][3][MAXQ][32 lanes]
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    const int64_t nrows = (int64_t)p.batch * p.seqlen;
-    // persistent warps, contiguous partition: warp i owns rows [i * per, (i + 1) * per) -- equal work for every warp and at
-    // most one batch boundary inside a range, so the per-batch sums are flushed once or twice per warp
-    const int64_t per = (nrows + nwarps - 1) / nwarps;
-    const int D = p.dim, nq = D >> 2;
-    const float invD = 1.f / D;
-    const T *nw = reinterpret_cast<const T *>(p.norm_w);
-    float w[MAXQ][4], acc_w[MAXQ][4];
-#pragma unroll
-    for (int k = 0; k < MAXQ; ++k) {
-        const int q = lane + 32 * k;
-        if (q < nq) ld4<T>(nw, 4 * q, w[k]);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) acc_w[k][i] = 0.f;
-#pragma unroll
-        for (int j = 0; j < 3; ++j) acc_s[(j * MAXQ + k) * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    auto flush_batch = [&](int b) {
-#pragma unroll
-        for (int k = 0; k < MAXQ; ++k) {
-            const int q = lane + 32 * k;
-            if (q < nq) {
-                float *dst[3] = {p.dgate, p.dshift, p.dscale};
-#pragma unroll
-                for (int j = 0; j < 3; ++j) {
-                    const float4 v = acc_s[(j * MAXQ + k) * 32];
-                    if (DET && dst[j]) {
-                        *reinterpret_cast<float4 *>(dst[j] + ((warp % (nwarps / p.batch)) * p.batch + b) * D + 4 * q) = v;
-                    } else if (dst[j]) {
-                        float *o = dst[j] + (int64_t)b * D + 4 * q;
-                        atomicAdd(o, v.x); atomicAdd(o + 1, v.y); atomicAdd(o + 2, v.z); atomicAdd(o + 3, v.w);
-                    }
-                    acc_s[(j * MAXQ + k) * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-            }
-        }
-    };
-    int64_t row0 = min(warp * per, nrows), row1 = min(row0 + per, nrows);
-    if constexpr (DET) {
-        const int64_t wpb = nwarps / p.batch, bw = warp / wpb, per_b = (p.seqlen + wpb - 1) / wpb;
-        row0 = row1 = nrows;
-        if (bw < p.batch) {
-            row0 = bw * p.seqlen + min((warp % wpb) * per_b, (int64_t)p.seqlen);
-            row1 = bw * p.seqlen + min((warp % wpb + 1) * per_b, (int64_t)p.seqlen);
-            if (row0 == row1) flush_batch((int)bw);      // no rows: this warp's partial rows are zeros
-        }
-    }
-    if (row0 < row1) {
-    int cur_b = (int)(row0 / p.seqlen);
-    for (int64_t row = row0; row < row1; ++row) {
-        const int b = (int)(row / p.seqlen), l = (int)(row % p.seqlen);
-        if (b != cur_b) { flush_batch(cur_b); cur_b = b; }
-        const int64_t mrow = (int64_t)b * p.seqlen + (p.rowmap ? p.rowmap[l] : l);
-        const float *r = p.r + row * D;
-        const T *dn = p.d_normed ? reinterpret_cast<const T *>(p.d_normed) + row * D : nullptr;
-        const T *dm = p.d_modded ? reinterpret_cast<const T *>(p.d_modded) + row * D : nullptr;
-        const float *dro = p.d_residual_out ? p.d_residual_out + row * D : nullptr;
-        const T *mix = p.mix ? reinterpret_cast<const T *>(p.mix) + mrow * D : nullptr;
-        const T *gate = p.gate ? reinterpret_cast<const T *>(p.gate) + (int64_t)b * p.mod_rs : nullptr;
-        const T *scale = p.scale ? reinterpret_cast<const T *>(p.scale) + (int64_t)b * p.mod_rs : nullptr;
-        const float rstd = p.rstd[row];
-        // ---- all streaming loads of the row first ----
-        float4 rr[MAXQ];
-        Raw4<T> rdn[MAXQ], rdm[MAXQ], rmx[MAXQ];
-#pragma unroll
-        for (int k = 0; k < MAXQ; ++k) {
-            const int q = lane + 32 * k;
-            if (q < nq) {
-                rr[k] = *reinterpret_cast<const float4 *>(r + 4 * q);
-                if (dn) rdn[k] = ldraw<T>(dn, 4 * q);
-                if (dm) rdm[k] = ldraw<T>(dm, 4 * q);
-                if (mix) rmx[k] = ldraw<T>(mix, 4 * q);
-            }
-        }
-        // ---- dy, per-column sums, c1 = mean(xhat * w * dy)  (xhat = r * rstd is recomputed where needed: registers) ----
-        float dy[MAXQ][4];
-        float c1 = 0.f;
-#pragma unroll
-        for (int k = 0; k < MAXQ; ++k) {
-            const int q = lane + 32 * k;
-            if (q < nq) {
-                const float xh[4] = {rr[k].x * rstd, rr[k].y * rstd, rr[k].z * rstd, rr[k].w * rstd};
-                float a[4] = {0.f, 0.f, 0.f, 0.f};
-                if (dn) cvt4<T>(rdn[k], a);
-                if (dm) {
-                    float sc[4], m[4];
-                    cvt4<T>(rdm[k], m);
-                    ld4<T>(scale, 4 * q, sc);
-                    float4 ash = acc_s[(1 * MAXQ + k) * 32], asc = acc_s[(2 * MAXQ + k) * 32];
-                    float *psh = &ash.x, *psc = &asc.x;
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        a[i] = fmaf(m[i], 1.f + sc[i], a[i]);
-                        psh[i] += m[i];
-                        psc[i] = fmaf(m[i], xh[i] * w[k][i], psc[i]);       // d_modded * normed
-                    }
-                    acc_s[(1 * MAXQ + k) * 32] = ash; acc_s[(2 * MAXQ + k) * 32] = asc;
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    dy[k][i] = a[i];
-                    acc_w[k][i] = fmaf(a[i], xh[i], acc_w[k][i]);
-                    c1 = fmaf(xh[i], a[i] * w[k][i], c1);
-                }
-            }
-        }
-        c1 = zg_warp_sum(c1) * invD;
-        // ---- dr, outputs ----
-        float *drin = p.d_residual_in ? p.d_residual_in + row * D : nullptr;
-        T *dx = reinterpret_cast<T *>(p.d_x) + row * D;
-        T *dmix = p.d_mix ? reinterpret_cast<T *>(p.d_mix) + mrow * D : nullptr;
-#pragma unroll
-        for (int k = 0; k < MAXQ; ++k) {
-            const int q = lane + 32 * k;
-            if (q < nq) {
-                const float xh[4] = {rr[k].x * rstd, rr[k].y * rstd, rr[k].z * rstd, rr[k].w * rstd};
-                float dr[4], dh[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) dr[i] = (dy[k][i] * w[k][i] - xh[i] * c1) * rstd;
-                if (dro) {
-                    const float4 t = *reinterpret_cast<const float4 *>(dro + 4 * q);
-                    dr[0] += t.x; dr[1] += t.y; dr[2] += t.z; dr[3] += t.w;
-                }
-                if (drin) st4<float>(drin, 4 * q, dr);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) dh[i] = round_to<T>(dr[i]);
-                st4<T>(dx, 4 * q, dh);
-                if (mix) {
-                    float m[4], g[4], o[4];
-                    cvt4<T>(rmx[k], m);
-                    ld4<T>(gate, 4 * q, g);
-                    float4 ag = acc_s[(0 * MAXQ + k) * 32];
-                    float *pg = &ag.x;
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) { o[i] = g[i] * dh[i]; pg[i] = fmaf(dh[i], m[i], pg[i]); }
-                    acc_s[(0 * MAXQ + k) * 32] = ag;
-                    st4<T>(dmix, 4 * q, o);
-                }
-            }
-        }
-    }
-    flush_batch(cur_b);
-    }
-    // d_norm_w: sum over the CTA's 4 warps in shared memory, then ONE plain store per column into this CTA's row of the
-    // (gridDim.x, dim) partials buffer -- atomics from every warp onto the same 640 addresses serialised for ~50 us
-    // (first version, 126 us per call); the caller adds the few hundred partial rows up.
-    if (p.d_norm_w) {
-        __syncthreads();
-        float *red = tailb_smem;                           // [4][4 * 32 * MAXQ]
-#pragma unroll
-        for (int k = 0; k < MAXQ; ++k)
-            *reinterpret_cast<float4 *>(red + (threadIdx.x >> 5) * (128 * MAXQ) + 4 * (lane + 32 * k)) = make_float4(acc_w[k][0], acc_w[k][1], acc_w[k][2], acc_w[k][3]);
-        __syncthreads();
-        for (int c = threadIdx.x; c < D; c += 128)
-            p.d_norm_w[(int64_t)blockIdx.x * D + c] = red[c] + red[128 * MAXQ + c] + red[2 * 128 * MAXQ + c] + red[3 * 128 * MAXQ + c];
-    }
+    constexpr bool DP = false;
+    [[maybe_unused]] const void *const path_scale = nullptr;
+#include "block_tail_bwd_body.cuh"
 }
 
-template <typename T, bool DET> static int block_tail_bwd_t(const zg_block_tail_bwd_params &p, cudaStream_t s) {
+template <typename T, int MAXQ, bool DET>
+__global__ void __launch_bounds__(128, 3) block_tail_dp_bwd_kernel(const zg_block_tail_bwd_dp_params q) {
+    constexpr bool DP = true;
+    const zg_block_tail_bwd_params &p = q.base;
+    const void *const path_scale = q.path_scale;
+#include "block_tail_bwd_body.cuh"
+}
+
+// path_scale NULL: block_tail_bwd_kernel; otherwise block_tail_dp_bwd_kernel (same MAXQ buckets, grid and shared memory)
+template <typename T, bool DET> static int block_tail_bwd_t(const zg_block_tail_bwd_params &p, const void *path_scale, cudaStream_t s) {
     const unsigned grid = (unsigned)p.nparts;          // persistent: the caller sized the d_norm_w partials buffer
     // dynamic shared memory: 4 warps x 3 accumulator sets x MAXQ quads x 32 lanes x 16 B  (<= 48 KB for MAXQ <= 8)
-    if (p.dim <= 512) block_tail_bwd_kernel<T, 4, DET><<<grid, 128, 4 * 3 * 4 * 32 * 16, s>>>(p);
-    else if (p.dim <= 640) block_tail_bwd_kernel<T, 5, DET><<<grid, 128, 4 * 3 * 5 * 32 * 16, s>>>(p);
-    else if (p.dim <= 768) block_tail_bwd_kernel<T, 6, DET><<<grid, 128, 4 * 3 * 6 * 32 * 16, s>>>(p);
-    else block_tail_bwd_kernel<T, 8, DET><<<grid, 128, 4 * 3 * 8 * 32 * 16, s>>>(p);
+#define ZG_TAILB(Q)                                                                                                             \
+    do {                                                                                                                        \
+        if (path_scale) block_tail_dp_bwd_kernel<T, Q, DET><<<grid, 128, 4 * 3 * Q * 32 * 16, s>>>(zg_block_tail_bwd_dp_params{p, path_scale}); \
+        else block_tail_bwd_kernel<T, Q, DET><<<grid, 128, 4 * 3 * Q * 32 * 16, s>>>(p);                                          \
+    } while (0)
+    if (p.dim <= 512) ZG_TAILB(4);
+    else if (p.dim <= 640) ZG_TAILB(5);
+    else if (p.dim <= 768) ZG_TAILB(6);
+    else ZG_TAILB(8);
+#undef ZG_TAILB
     zg_count_launch();
-    return zg_check_launch("block_tail_bwd");
+    return zg_check_launch(path_scale ? "block_tail_bwd_dp" : "block_tail_bwd");
 }
 
 template <typename T, typename R> static int norm_fwd_tr(const zg_norm_params &p, cudaStream_t s) {
@@ -917,9 +801,7 @@ extern "C" int zg_add_norm_bwd_det(const zg_norm_bwd_params *pp, void *workspace
     return lay.reduce(s);
 }
 
-static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bool pe) {
-    ZG_REQUIRE(pp != nullptr, "block_tail_fwd: null params");
-    const zg_block_tail_params &p = *pp;
+static int block_tail_fwd_validate(const zg_block_tail_params &p, bool pe) {
     ZG_REQUIRE(p.x && p.norm_w && p.normed, "block_tail_fwd: null tensor pointer");
     if (pe) ZG_REQUIRE(p.mix && !p.gate && !p.rowmap && !p.residual, "block_tail_fwd_pe: takes the (seqlen, dim) table as mix and no gate / rowmap / residual");
     else ZG_REQUIRE(!p.mix || p.gate, "block_tail_fwd: mix needs gate");
@@ -931,6 +813,13 @@ static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bo
                "block_tail_fwd: row tensors must be 16-byte aligned");
     ZG_REQUIRE(aligned_quad(p.gate, p.dtype) && aligned_quad(p.shift, p.dtype) && aligned_quad(p.scale, p.dtype) && aligned_quad(p.norm_w, p.dtype),
                "block_tail_fwd: gate / shift / scale / norm_w must be aligned to 4 elements");
+    return 0;
+}
+
+static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bool pe) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_fwd: null params");
+    const zg_block_tail_params &p = *pp;
+    if (int rc = block_tail_fwd_validate(p, pe)) return rc;
     const int64_t nrows = (int64_t)p.batch * p.seqlen;
     if (nrows == 0) return 0;
     cudaStream_t s = (cudaStream_t)stream;
@@ -944,6 +833,32 @@ static int block_tail_fwd_entry(const zg_block_tail_params *pp, void *stream, bo
 
 extern "C" int zg_block_tail_fwd(const zg_block_tail_params *pp, void *stream) { return block_tail_fwd_entry(pp, stream, false); }
 extern "C" int zg_block_tail_fwd_pe(const zg_block_tail_params *pp, void *stream) { return block_tail_fwd_entry(pp, stream, true); }
+
+// path_scale is read as one dtype element per batch element
+static bool aligned_elem(const void *p, int dtype) {
+    return (reinterpret_cast<uintptr_t>(p) & ((dtype == ZG_F32 ? sizeof(float) : sizeof(__half)) - 1)) == 0;
+}
+
+extern "C" int zg_block_tail_fwd_dp(const zg_block_tail_dp_params *pp, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_fwd_dp: null params");
+    const zg_block_tail_params &p = pp->base;
+    ZG_REQUIRE(pp->path_scale != nullptr, "block_tail_fwd_dp: null path_scale");
+    ZG_REQUIRE(p.residual != nullptr && p.mix != nullptr, "block_tail_fwd_dp: needs residual and mix (the first block has no drop path)");
+    ZG_REQUIRE(p.final_layer == 0, "block_tail_fwd_dp: final_layer is not supported");
+    ZG_REQUIRE(p.dim <= 1024, "block_tail_fwd_dp: dim must be <= 1024, got %d", p.dim);
+    if (int rc = block_tail_fwd_validate(p, false)) return rc;
+    ZG_REQUIRE(aligned_elem(pp->path_scale, p.dtype), "block_tail_fwd_dp: path_scale must be aligned to its element size");
+    const int64_t nrows = (int64_t)p.batch * p.seqlen;
+    if (nrows == 0) return 0;
+    ZG_REQUIRE(nrows <= 0x7fffffffLL, "block_tail_fwd_dp: fewer than 2^31 rows only");
+    cudaStream_t s = (cudaStream_t)stream;
+    switch (p.dtype) {
+        case ZG_F32: return zg::block_tail_dp_t<float>(*pp, s);
+        case ZG_F16: return zg::block_tail_dp_t<__half>(*pp, s);
+        case ZG_BF16: return zg::block_tail_dp_t<__nv_bfloat16>(*pp, s);
+    }
+    return zg_set_error("block_tail_fwd_dp: bad dtype %d", p.dtype);
+}
 
 static int block_tail_bwd_validate(const zg_block_tail_bwd_params &p) {
     ZG_REQUIRE(p.r && p.rstd && p.norm_w && p.d_x, "block_tail_bwd: null tensor pointer");
@@ -961,11 +876,11 @@ static int block_tail_bwd_validate(const zg_block_tail_bwd_params &p) {
     return 0;
 }
 
-template <bool DET> static int block_tail_bwd_dispatch(const zg_block_tail_bwd_params &p, cudaStream_t s) {
+template <bool DET> static int block_tail_bwd_dispatch(const zg_block_tail_bwd_params &p, const void *path_scale, cudaStream_t s) {
     switch (p.dtype) {
-        case ZG_F32: return zg::block_tail_bwd_t<float, DET>(p, s);
-        case ZG_F16: return zg::block_tail_bwd_t<__half, DET>(p, s);
-        default: return zg::block_tail_bwd_t<__nv_bfloat16, DET>(p, s);
+        case ZG_F32: return zg::block_tail_bwd_t<float, DET>(p, path_scale, s);
+        case ZG_F16: return zg::block_tail_bwd_t<__half, DET>(p, path_scale, s);
+        default: return zg::block_tail_bwd_t<__nv_bfloat16, DET>(p, path_scale, s);
     }
 }
 
@@ -973,7 +888,23 @@ extern "C" int zg_block_tail_bwd(const zg_block_tail_bwd_params *pp, void *strea
     ZG_REQUIRE(pp != nullptr, "block_tail_bwd: null params");
     if (int rc = block_tail_bwd_validate(*pp)) return rc;
     if (pp->batch == 0 || pp->seqlen == 0) return 0;
-    return block_tail_bwd_dispatch<false>(*pp, (cudaStream_t)stream);
+    return block_tail_bwd_dispatch<false>(*pp, nullptr, (cudaStream_t)stream);
+}
+
+// the drop-path backward takes everything the plain one takes, plus a path_scale; a block without mix has no drop path
+static int block_tail_bwd_dp_validate(const zg_block_tail_bwd_dp_params *pp) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_bwd_dp: null params");
+    ZG_REQUIRE(pp->path_scale != nullptr, "block_tail_bwd_dp: null path_scale");
+    ZG_REQUIRE(pp->base.mix != nullptr, "block_tail_bwd_dp: needs mix (the first block has no drop path)");
+    if (int rc = block_tail_bwd_validate(pp->base)) return rc;
+    ZG_REQUIRE(aligned_elem(pp->path_scale, pp->base.dtype), "block_tail_bwd_dp: path_scale must be aligned to its element size");
+    return 0;
+}
+
+extern "C" int zg_block_tail_bwd_dp(const zg_block_tail_bwd_dp_params *pp, void *stream) {
+    if (int rc = block_tail_bwd_dp_validate(pp)) return rc;
+    if (pp->base.batch == 0 || pp->base.seqlen == 0) return 0;
+    return block_tail_bwd_dispatch<false>(pp->base, pp->path_scale, (cudaStream_t)stream);
 }
 
 // partial rows of the deterministic backward: one per warp index within a batch element (see block_tail_bwd_kernel)
@@ -992,20 +923,35 @@ extern "C" int64_t zg_block_tail_bwd_det_workspace_bytes(const zg_block_tail_bwd
     return p ? block_tail_bwd_det_layout(*p, nullptr).bytes : 0;
 }
 
-extern "C" int zg_block_tail_bwd_det(const zg_block_tail_bwd_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
-    ZG_REQUIRE(pp != nullptr, "block_tail_bwd_det: null params");
-    if (int rc = block_tail_bwd_validate(*pp)) return rc;
-    if (pp->batch == 0 || pp->seqlen == 0) return 0;
-    ZG_REQUIRE(4 * (int64_t)pp->nparts >= pp->batch, "block_tail_bwd_det: needs at least one warp per batch element (4 * nparts >= batch), got nparts %d for batch %d",
-               pp->nparts, pp->batch);
-    const ZgDetLayout lay = block_tail_bwd_det_layout(*pp, workspace);
+// validated params; path_scale NULL for the plain entry point
+static int block_tail_bwd_det_run(const zg_block_tail_bwd_params &q, const void *path_scale, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (q.batch == 0 || q.seqlen == 0) return 0;
+    ZG_REQUIRE(4 * (int64_t)q.nparts >= q.batch, "block_tail_bwd_det: needs at least one warp per batch element (4 * nparts >= batch), got nparts %d for batch %d",
+               q.nparts, q.batch);
+    const ZgDetLayout lay = block_tail_bwd_det_layout(q, workspace);
     ZG_REQUIRE_WORKSPACE(lay, workspace, workspace_bytes, "block_tail_bwd_det");
-    zg_block_tail_bwd_params p = *pp;           // the kernel writes partial rows; the reduction adds them to the outputs
+    zg_block_tail_bwd_params p = q;             // the kernel writes partial rows; the reduction adds them to the outputs
     int i = 0;
     if (p.dgate) p.dgate = lay.reg[i++].part;
     if (p.dshift) p.dshift = lay.reg[i++].part;
     if (p.dscale) p.dscale = lay.reg[i++].part;
     cudaStream_t s = (cudaStream_t)stream;
-    if (int rc = block_tail_bwd_dispatch<true>(p, s)) return rc;
+    if (int rc = block_tail_bwd_dispatch<true>(p, path_scale, s)) return rc;
     return lay.reduce(s);
+}
+
+extern "C" int zg_block_tail_bwd_det(const zg_block_tail_bwd_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_bwd_det: null params");
+    if (int rc = block_tail_bwd_validate(*pp)) return rc;
+    return block_tail_bwd_det_run(*pp, nullptr, workspace, workspace_bytes, stream);
+}
+
+// the multiplier does not touch any column sum's layout: the same partials as the plain deterministic backward
+extern "C" int64_t zg_block_tail_bwd_dp_det_workspace_bytes(const zg_block_tail_bwd_dp_params *p) {
+    return p ? block_tail_bwd_det_layout(p->base, nullptr).bytes : 0;
+}
+
+extern "C" int zg_block_tail_bwd_dp_det(const zg_block_tail_bwd_dp_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
+    if (int rc = block_tail_bwd_dp_validate(pp)) return rc;
+    return block_tail_bwd_det_run(pp->base, pp->path_scale, workspace, workspace_bytes, stream);
 }

@@ -55,11 +55,15 @@ def scan_hot_path_ok(dtype, E, L, N, R):
 
 
 def block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, final=False, mod_div=1, want_modded=True, want_rstd=False,
-               mix_bcast=False):
+               mix_bcast=False, path_scale=None):
     """zg_block_tail_fwd wrapper.  x: (Bt, L, D) contiguous; gate/shift/scale: (Bt // mod_div, D)
     views with a common row stride.  Returns residual_out (fp32), normed, modded.
-    mix_bcast: ``mix`` is one (L, D) table added to every batch element (gate None = 1): the positional embedding."""
-    _lib.require_cuda(x, mix, gate, shift, scale, norm_w, residual, rowmap)
+    mix_bcast: ``mix`` is one (L, D) table added to every batch element (gate None = 1): the positional embedding.
+    path_scale: (Bt,) drop-path multipliers in x.dtype (zg_block_tail_fwd_dp): hidden * path_scale[b] joins the residual."""
+    _lib.require_cuda(x, mix, gate, shift, scale, norm_w, residual, rowmap, path_scale)
+    if path_scale is not None and (path_scale.dtype != x.dtype or tuple(path_scale.shape) != (x.shape[0],) or not path_scale.is_contiguous()):
+        raise RuntimeError(f"block_tail: path_scale must be a contiguous ({x.shape[0]},) tensor in {x.dtype}, got "
+                           f"{tuple(path_scale.shape)} {path_scale.dtype}")
     Bt, L, D = x.shape
     if mod_div != 1:
         # modulation vectors are per ORIGINAL batch element; expand to the folded batch (tiny)
@@ -107,7 +111,10 @@ def block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, final=
     p.rstd = _lib.ptr(rstd)
     if mix_bcast and (mix is None or mix.numel() != L * D or gate is not None or rowmap is not None or residual is not None):
         raise RuntimeError("block_tail: mix_bcast takes a (seqlen, dim) mix table and no gate / rowmap / residual")
-    _lib.call("zg_block_tail_fwd_pe" if mix_bcast else "zg_block_tail_fwd", p)
+    if path_scale is not None:
+        _lib.call("zg_block_tail_fwd_dp", _lib.BlockTailDpParams(p, _lib.ptr(path_scale)))
+    else:
+        _lib.call("zg_block_tail_fwd_pe" if mix_bcast else "zg_block_tail_fwd", p)
     if want_rstd:
         return res_out, normed, modded, rstd
     return res_out, normed, modded

@@ -94,14 +94,19 @@ class DropPath(nn.Module):
         super().__init__()
         self.drop_prob, self.scale_by_keep = drop_prob, scale_by_keep
 
-    def forward(self, x):
-        if self.drop_prob == 0.0 or not self.training:
-            return x
+    def draw(self, x):
+        """The per-sample multipliers, (B, 1, ..., 1) in x's dtype: 0 or 1 / keep (rounded to the dtype).  The fused training
+        tail (ZigMa._forward_fused_tail) takes them from here too, so both paths make the same generator calls."""
         keep = 1 - self.drop_prob
         mask = x.new_empty((x.shape[0],) + (1,) * (x.ndim - 1)).bernoulli_(keep)
         if keep > 0.0 and self.scale_by_keep:
             mask.div_(keep)
-        return x * mask
+        return mask
+
+    def forward(self, x):
+        if self.drop_prob == 0.0 or not self.training:
+            return x
+        return x * self.draw(x)
 
 
 class TimestepEmbedder(nn.Module):
@@ -430,19 +435,20 @@ class ZigMa(nn.Module):
                 and isinstance(self.norm_f, RMSNorm))
 
     def _fused_tail_ok(self, hidden_states):
-        """The fused training loop (block_ops.BlockTailFn) covers the configuration every shipped config uses."""
+        """The fused training loop (block_ops.BlockTailFn) covers the configuration every shipped config uses, in eval and in
+        train mode (stochastic depth included)."""
         import os
         D = hidden_states.shape[-1]
         return (hidden_states.is_cuda and self.fused_add_norm and self.residual_in_fp32 and not self.has_text and self.use_pe != 3
                 and not self.use_checkpoint and D % 4 == 0 and D <= 1024 and hidden_states.dtype in (torch.float32, torch.bfloat16, torch.float16)
-                and all(isinstance(b.norm, RMSNorm) and b.skip_linear is None and (isinstance(b.drop_path, nn.Identity) or not b.training)
-                        for b in self.blocks)
-                and isinstance(self.norm_f, RMSNorm) and (isinstance(self.drop_path, nn.Identity) or not self.training)
-                and os.environ.get("ZIGMA_FUSED_TRAIN_TAIL", "1") != "0")
+                and all(isinstance(b.norm, RMSNorm) and b.skip_linear is None for b in self.blocks)
+                and isinstance(self.norm_f, RMSNorm) and os.environ.get("ZIGMA_FUSED_TRAIN_TAIL", "1") != "0")
 
     def _forward_fused_tail(self, hidden_states, c):
         """Same function as the block loop of forward_autograd: each block's add+norm+modulate and the PREVIOUS block's
-        gated residual add + un-permutation run as one kernel (forward and backward)."""
+        gated residual add + un-permutation run as one kernel (forward and backward).  A block with an active DropPath
+        (training, drop_prob > 0, a residual to join) draws its multipliers here, at the point Block.forward would, and
+        its tail applies them (block_tail_fn's path_scale)."""
         from .block_ops import block_tail_fn
         from .mamba_simple import permute_along
         residual, mix, gate, rowmap = None, None, None, None
@@ -450,7 +456,12 @@ class ZigMa(nn.Module):
         for block in self.blocks:
             mods = block.adaLN_modulation(c)
             shift, scale, gate_next = mods.chunk(3, dim=1)
-            residual, x, modded = block_tail_fn(x, mix, gate, shift, scale, block.norm.weight, residual, rowmap, block.norm.eps)
+            dp = block.drop_path
+            path_scale = None
+            if residual is not None and isinstance(dp, DropPath) and dp.training and dp.drop_prob > 0.0:
+                path_scale = dp.draw(x).reshape(x.shape[0])     # x: the dtype the kernel forms hidden in
+            residual, x, modded = block_tail_fn(x, mix, gate, shift, scale, block.norm.weight, residual, rowmap, block.norm.eps,
+                                                path_scale)
             mix, rowmap = block.mixer.forward_scan_order(modded)
             gate = gate_next
         if rowmap is not None:
