@@ -12,76 +12,19 @@ The references take exactly the values the kernels read (inputs are drawn in the
 * column sums (weight / bias / modulation gradients): |a - e| <= 1e-5 * S + one ulp of the returned dtype, S = sum of |term|
   over the summed rows; test_column_sum_bound_rejects_a_dropped_row shows that losing one row breaks it.
 The achieved ulps, mismatch fractions and fp32 constants go to $ZIGMA_PARITY_LOG when it names a file."""
-import json
-import os
 import re
 
 import pytest
 import torch
 
+from util import COLSUM_REL, DTYPE_NAME, check_colsum, check_elem, ulp
+
 DEV = "cuda"
 gpu = pytest.mark.gpu
 
-C_F32 = 64                                  # fp32 bound: |a - e| <= C_F32 * 2^-24 * M
-COLSUM_REL = 1e-5
-MISMATCH = {torch.float16: 5e-3, torch.bfloat16: 1e-3}      # measured on an H100: at most 1.2e-3 and 2e-4
-MANT = {torch.float16: 10, torch.bfloat16: 7, torch.float32: 23}
 LOWP = (torch.float16, torch.bfloat16)
 DTYPES = (torch.float32, torch.float16, torch.bfloat16)
-_NAME = {torch.float32: "fp32", torch.float16: "fp16", torch.bfloat16: "bf16"}
-
-
-# ------------------------------------------------------------------------------------------------ comparison
-def ulp(e, dtype):
-    """Unit in the last place of `dtype` at the fp64 values e (the subnormal spacing below the normal range)."""
-    _, ex = torch.frexp(e.abs())
-    u = torch.ldexp(torch.ones_like(e), ex - 1 - MANT[dtype])
-    floor = torch.finfo(dtype).tiny * 2.0 ** -MANT[dtype]
-    return torch.where(e == 0, torch.full_like(e, floor), u.clamp(min=floor))
-
-
-def _log(what, dtype, **rec):
-    path = os.environ.get("ZIGMA_PARITY_LOG")
-    if path:
-        rec = dict(test=os.environ.get("PYTEST_CURRENT_TEST", "").split(" ")[0], what=what, dtype=_NAME[dtype], **rec)
-        with open(path, "a") as f:
-            f.write(json.dumps(rec) + "\n")
-
-
-def check_elem(what, a, e, M, max_ulp=1, extra=None):
-    """a: kernel output; e: fp64 reference before the output's final rounding; M: fp64 magnitude of the terms of each element.
-    extra (16-bit chained outputs whose rounded intermediate is not an output): what a one-ulp difference of that intermediate
-    moves the element by, added to the cancellation allowance."""
-    dtype = a.dtype
-    a = a.detach().double().cpu()
-    assert a.shape == e.shape, f"{what}: shape {tuple(a.shape)} vs {tuple(e.shape)}"
-    assert torch.isfinite(a).all(), f"{what}: non-finite values"
-    diff = (a - e).abs()
-    fp32_bound = C_F32 * 2.0 ** -24 * M
-    c = (diff / M.clamp(min=1e-300) / 2.0 ** -24).max().item() if a.numel() else 0.0
-    if dtype == torch.float32:
-        bad = diff > fp32_bound
-        _log(what, dtype, worst_c=c, numel=a.numel())
-        assert not bad.any(), f"{what}: {int(bad.sum())}/{a.numel()} beyond {C_F32}*2^-24*M (worst c {c:.1f})"
-        return
-    u = ulp(e, dtype)
-    dist = diff / u
-    bad = (dist > max_ulp) & (diff > fp32_bound + u + (0 if extra is None else extra))
-    mism = (a != e.to(dtype).double()).double().mean().item()
-    worst = dist.max().item() if a.numel() else 0.0
-    _log(what, dtype, max_ulp=worst, mismatch_frac=mism, numel=a.numel())
-    assert not bad.any(), f"{what}: {int(bad.sum())}/{a.numel()} elements beyond {max_ulp} ulp (worst {worst:.2f} ulp)"
-    assert mism <= MISMATCH[dtype], f"{what}: {mism:.2e} of the elements differ from the rounded reference"
-
-
-def check_colsum(what, a, e, S):
-    dtype = a.dtype
-    ad = a.detach().double().cpu()
-    assert ad.shape == e.shape and torch.isfinite(ad).all(), what
-    bound = COLSUM_REL * S + ulp(e, dtype)
-    worst = ((ad - e).abs() / bound).max().item()
-    _log(what, dtype, colsum_worst_frac_of_bound=worst, numel=ad.numel())
-    assert worst <= 1.0, f"{what}: column sum off by {worst:.2f} x (1e-5 S + 1 ulp)"
+_NAME = DTYPE_NAME
 
 
 def test_column_sum_bound_rejects_a_dropped_row():

@@ -68,6 +68,78 @@ def _log_parity(what, max_diff, max_ref, strict, hard_viol, numel, rtol, atol, m
         pass
 
 
+# ------------------------------------------------------------------------------------------------ bounds against fp64 references
+# Shared by the kernel-against-fp64 files (test_gpu_norm_kernels.py, test_gpu_scan_kernels.py).  a: kernel output; e: the fp64
+# reference before the output's final rounding; M: the fp64 magnitude of the terms that form each element (never |e|, which is
+# small exactly where the terms cancel); S: the sum of |term| over what a reduced output sums.
+MANT = {torch.float16: 10, torch.bfloat16: 7, torch.float32: 23}
+DTYPE_NAME = {torch.float32: "fp32", torch.float16: "fp16", torch.bfloat16: "bf16"}
+C_F32 = 64                                  # fp32 elements: |a - e| <= c_f32 * 2^-24 * M (+ the smallest normal fp32)
+COLSUM_REL = 1e-5                           # sums: |a - e| <= rel * S + one ulp of the returned dtype
+MISMATCH = {torch.float16: 5e-3, torch.bfloat16: 1e-3}      # 16-bit: fraction of elements that differ from round(e)
+
+
+def ulp(e, dtype):
+    """Unit in the last place of `dtype` at the fp64 values e (the subnormal spacing below the normal range)."""
+    _, ex = torch.frexp(e.abs())
+    u = torch.ldexp(torch.ones_like(e), ex - 1 - MANT[dtype])
+    floor = torch.finfo(dtype).tiny * 2.0 ** -MANT[dtype]
+    return torch.where(e == 0, torch.full_like(e, floor), u.clamp(min=floor))
+
+
+def _log(what, dtype, **rec):
+    path = os.environ.get("ZIGMA_PARITY_LOG")
+    if path:
+        rec = dict(test=os.environ.get("PYTEST_CURRENT_TEST", "").split(" ")[0], what=what, dtype=DTYPE_NAME[dtype], **rec)
+        with open(path, "a") as f:
+            f.write(json.dumps(rec) + "\n")
+
+
+def check_elem(what, a, e, M, max_ulp=1, extra=None, c_f32=C_F32, mismatch=None, conditioned=False):
+    """Elementwise bound.  fp32: |a - e| <= c_f32 * 2^-24 * M + the smallest normal fp32 (a result that underflows may flush).
+    16-bit: at most max_ulp ulps of e, or, for an element formed by cancellation, the fp32 bound plus one ulp (plus `extra`:
+    what a one-ulp difference of a rounded intermediate that is not an output moves the element by); and the fraction of
+    elements that differ from round(e) stays below mismatch (default MISMATCH[dtype]); conditioned: among the elements whose
+    fp32 allowance is under a quarter ulp only."""
+    dtype = a.dtype
+    a = a.detach().double().to(e.device)
+    assert a.shape == e.shape, f"{what}: shape {tuple(a.shape)} vs {tuple(e.shape)}"
+    assert torch.isfinite(a).all(), f"{what}: non-finite values"
+    diff = (a - e).abs()
+    fp32_bound = c_f32 * 2.0 ** -24 * M + torch.finfo(torch.float32).tiny
+    c = (diff / M.clamp(min=1e-300) / 2.0 ** -24).max().item() if a.numel() else 0.0
+    if dtype == torch.float32:
+        bad = diff > fp32_bound
+        _log(what, dtype, worst_c=c, frac_of_bound=(diff / fp32_bound).max().item() if a.numel() else 0.0, numel=a.numel())
+        assert not bad.any(), f"{what}: {int(bad.sum())}/{a.numel()} beyond {c_f32}*2^-24*M (worst c {c:.1f})"
+        return
+    u = ulp(e, dtype)
+    dist = diff / u
+    allow = torch.maximum(max_ulp * u, fp32_bound + u + (0 if extra is None else extra))
+    bad = diff > allow
+    # the mismatch fraction counts the elements whose fp32 allowance is under a quarter ulp (or all, conditioned=False): where
+    # long accumulation or cancellation makes M large against |e|, a differing last bit says nothing about a rounding point
+    cond = (fp32_bound <= 0.25 * u) if conditioned else torch.ones_like(u, dtype=torch.bool)
+    mism = (a != e.to(dtype).double())[cond].double().mean().item() if cond.any() else 0.0
+    worst = dist.max().item() if a.numel() else 0.0
+    _log(what, dtype, max_ulp=worst, frac_of_bound=(diff / allow).max().item() if a.numel() else 0.0, mismatch_frac=mism, numel=a.numel())
+    assert not bad.any(), f"{what}: {int(bad.sum())}/{a.numel()} elements beyond {max_ulp} ulp (worst {worst:.2f} ulp)"
+    limit = MISMATCH[dtype] if mismatch is None else mismatch
+    assert mism <= limit, f"{what}: {mism:.2e} of the elements differ from the rounded reference"
+
+
+def check_colsum(what, a, e, S, rel=COLSUM_REL):
+    """Reduced outputs (weight / bias / modulation gradients, sums over rows or channels): |a - e| <= rel * S + one ulp
+    (+ the smallest normal fp32)."""
+    dtype = a.dtype
+    ad = a.detach().double().to(e.device)
+    assert ad.shape == e.shape and torch.isfinite(ad).all(), what
+    bound = rel * S + ulp(e, dtype) + torch.finfo(torch.float32).tiny     # (fp32 accumulation flushes subnormal terms)
+    worst = ((ad - e).abs() / bound).max().item() if ad.numel() else 0.0
+    _log(what, dtype, colsum_worst_frac_of_bound=worst, numel=ad.numel())
+    assert worst <= 1.0, f"{what}: sum off by {worst:.2f} x ({rel:g} S + 1 ulp)"
+
+
 def model_case(name):
     g = gold("model_" + name)
     cfg = json.loads(bytes(g["cfg_json"]).decode())

@@ -153,7 +153,7 @@ __global__ void __launch_bounds__(BWD_CH) scan_bwd_kernel(const zg_scan_bwd_para
                     red[n] = dhn * d * u_;
                     red[NS + n] = dy * hl;
                 }
-                if (softplus) dd *= (1.f - __expf(-d));       // sigmoid(delta~) = 1 - exp(-softplus(delta~))
+                if (softplus) dd *= zg_softplus_grad(d);     // sigmoid(delta~) = 1 - exp(-softplus(delta~))
                 dbias_acc += dd;
                 if (active) {
                     gdu[l] = zg_from_float<T>(du_);

@@ -298,7 +298,7 @@ __global__ void __launch_bounds__(Q4_THREADS, 4) scan_bwd_q4_kernel(const zg_sca
                 if (qd == 0) {
                     const float du_ = fmaf(s.x, s1q, s.z * Dv);
                     float dd = fmaf(s2q, ZG_LN2, s.y * s1q);
-                    if (softplus) dd *= 1.f - zg_ex2(-s.x * ZG_LOG2E);   // sigmoid(delta~) = 1 - exp(-softplus(delta~))
+                    if (softplus) dd *= zg_softplus_grad(s.x);   // sigmoid(delta~) = 1 - exp(-softplus(delta~))
                     dD_acc = fmaf(s.z, s.y, dD_acc);
                     dbias_acc += dd;
                     *scp = make_float4(du_, dd, s.w * fmaf(Dv, s.y, yq), 0.f);   // the slot now carries the outputs

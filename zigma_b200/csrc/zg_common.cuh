@@ -98,6 +98,13 @@ __device__ __forceinline__ float zg_softplus20(float x) {
     return (x > 20.f) ? x : sp;
 }
 
+// softplus'(x) = sigmoid(x) = 1 - exp(-softplus(x)), from sp = softplus(x) (the value the scan already holds).  Below
+// sp = 1/8 (x below about -2) the difference 1 - exp(-sp) cancels -- at x = -30 it is 0 in fp32, where sigmoid(x) = 9e-14 --
+// so there it is the series sp (1 - sp/2 (1 - sp/3 (1 - sp/4 (1 - sp/5 (1 - sp/6))))), relative error < sp^6 / 5040 < 1e-9.
+__device__ __forceinline__ float zg_softplus_grad(float sp) {
+    const float series = sp * (1.f - 0.5f * sp * (1.f - sp * (1.f / 3.f) * (1.f - 0.25f * sp * (1.f - 0.2f * sp * (1.f - sp * (1.f / 6.f))))));
+    return sp < 0.125f ? series : 1.f - zg_ex2(-sp * ZG_LOG2E);
+}
 __device__ __forceinline__ float zg_sigmoid(float x) { return zg_rcp(1.f + zg_ex2(-x * ZG_LOG2E)); }
 __device__ __forceinline__ float zg_silu(float x) { return x * zg_sigmoid(x); }
 

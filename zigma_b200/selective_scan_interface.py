@@ -177,7 +177,9 @@ def _scan_bwd(saved, ckpt, dout, delta_softplus, dz_out=None, z_rowmap=None):
 
     def dense(t):      # the dstate == 16 kernel takes any strides; keep channel-first or token-major as given
         return t is None or t.stride(2) == 1 or t.stride(1) == 1
-    if dstate == 16 and var_b and var_c and all(dense(t) for t in (u, delta, z, dout)):
+    # (it also needs A and the checkpoints 16-byte aligned, scan_bwd_q4_fits; a contiguous A view 4 bytes off goes generic)
+    if (dstate == 16 and var_b and var_c and A.data_ptr() % 16 == 0 and ckpt.data_ptr() % 16 == 0
+            and all(dense(t) for t in (u, delta, z, dout))):
         fmt = torch.preserve_format
     else:              # generic kernel: a thread walks its own row, rows must be seq-contiguous
         def seqc(t):
