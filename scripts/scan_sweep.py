@@ -1,6 +1,6 @@
 """Times the selective-scan forward kernel at a layer shape (default BASELINE config 2: bs=64, E=1280, L=1024, N=16, bf16,
 token-major, z through the zigzag table).  The kernel choice is made by environment variables read once per process
-(ZG_SCAN_TMA, ZG_SCAN_TMA_NPOLY, ZG_SCAN_TPC2_NPOLY; ZG_SCAN_WP / ZG_SCAN_WP_WARPS / ZG_SCAN_WP_NPOLY are read per call): run once per setting.  FUSED=1 times the fused dt_proj prologue
+(ZG_SCAN_TMA, ZG_SCAN_PLAIN; ZG_SCAN_WP / ZG_SCAN_WPH_ND / ZG_SCAN_WPH_NS are read per call): run once per setting.  FUSED=1 times the fused dt_proj prologue
 (no delta tensor) next to the two-kernel route dt_proj GEMM + scan."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -40,7 +40,7 @@ def timeit(fn, n=20):
     return a.elapsed_time(b) / n
 t_tok = timeit(tok)
 abytes = 4 * 2 * bs * E * L + 2 * 2 * bs * N * L + 4 * (E * N + 2 * E)
-tag = " ".join(f"{k}={os.environ[k]}" for k in ("ZG_SCAN_TMA", "ZG_SCAN_PLAIN", "ZG_SCAN_TMA_NPOLY", "ZG_SCAN_TPC2_NPOLY", "ZG_SCAN_WP", "ZG_SCAN_WP_WARPS", "ZG_SCAN_WP_NPOLY", "ZG_SCAN_WP_SYNC", "ZG_SCAN_WPH_ND", "ZG_SCAN_WPH_NS", "ZIGMA_B200_LIB") if k in os.environ) or "default"
+tag = " ".join(f"{k}={os.environ[k]}" for k in ("ZG_SCAN_TMA", "ZG_SCAN_PLAIN", "ZG_SCAN_WP", "ZG_SCAN_WPH_ND", "ZG_SCAN_WPH_NS", "ZIGMA_B200_LIB") if k in os.environ) or "default"
 line = f"[{tag}] bs={bs} L={L} E={E}: scan {t_tok:.4f} ms ({abytes / t_tok / 1e6:.0f} GB/s of {abytes / 1e6:.0f} MB)"
 if os.environ.get("FUSED", "1") == "1" and R in (40, 48) and L % 8 == 0:
     t_gemm, t_fused = timeit(gemm), timeit(fused)

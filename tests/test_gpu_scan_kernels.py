@@ -14,21 +14,18 @@ The backward does the same on the reverse recurrence of dh.  The CPU tests below
 autograd and show that every bound rejects a kernel that drops one term.  The achieved fractions of the bounds go to
 $ZIGMA_PARITY_LOG when it names a file.
 
-The last part is the instantiation inventory: the table DEFAULT | OPT_IN lists every zg::scan_fwd* / zg::scan_bwd* kernel of the
-library; a CPU test holds it against the built library, and GPU tests check that the matrix launches exactly DEFAULT and that
-the environment switches launch exactly OPT_IN."""
+The last part is the instantiation inventory: the table DEFAULT lists every zg::scan_fwd* / zg::scan_bwd* kernel of the library;
+a CPU test holds it against the built library, and a GPU test checks that the matrix launches exactly DEFAULT."""
 import itertools
-import json
 import os
 import re
 import shutil
 import subprocess
-import sys
 
 import pytest
 import torch
 
-from util import DTYPE_NAME, ROOT, check_colsum, check_elem, ulp
+from util import DTYPE_NAME, check_colsum, check_elem, ulp
 
 DEV = "cuda"
 gpu = pytest.mark.gpu
@@ -708,49 +705,27 @@ T_16 = ("__half", "__nv_bfloat16")
 
 
 def _inventory():
-    """(kernel, template args) of every scan kernel of the library, split by whether a call reaches it from its inputs alone
-    (DEFAULT) or only under an environment switch (OPT_IN), from the dispatch code of scan_fwd*.cuh / scan_bwd*.cuh."""
-    dflt, opt = set(), set()
+    """(kernel, template args) of every scan kernel of the library, from the dispatch code of scan_fwd*.cuh / scan_bwd*.cuh: each
+    one is reached by some call's inputs alone."""
+    dflt = set()
     for t in T_ALL:                                    # generic forward: NS 8 / 16 / 32 / 64, both layouts; constant B / C <= 16
         for ns in (8, 16, 32, 64):
             for seq in (True, False):
-                dflt.add(("scan_fwd_kernel", (t, str(ns), _b(seq), "false", "0")))
+                dflt.add(("scan_fwd_kernel", (t, str(ns), _b(seq), "false")))
         for ns in (8, 16):
             for seq in (True, False):
-                dflt.add(("scan_fwd_kernel", (t, str(ns), _b(seq), "true", "0")))
-        for seq in (True, False):                      # ZG_SCAN_NPOLY = 2 / 3 / 4
-            for npoly in (2, 3, 4):
-                opt.add(("scan_fwd_kernel", (t, "16", _b(seq), "false", str(npoly))))
+                dflt.add(("scan_fwd_kernel", (t, str(ns), _b(seq), "true")))
     for t in T_16:
         # hot path: R 0 (plain = the model's call: z, softplus, no reverse / accumulate) and the fused dt_proj prologue R 40 / 48
-        for plain in (False, True):
-            for ck in (True, False):
-                dflt.add(("scan_fwd_tma_kernel", (t, "0", "0", _b(ck), "2", _b(plain))))
-            for npoly in (1, 2):                       # ZG_SCAN_TMA_NPOLY
-                opt.add(("scan_fwd_tma_kernel", (t, "0", str(npoly), "false", "2", _b(plain))))
-        for R in ("40", "48"):
-            for ck in (True, False):
-                dflt.add(("scan_fwd_tma_kernel", (t, R, "0", _b(ck), "2", "false")))
-            for npoly in (1, 2):
-                opt.add(("scan_fwd_tma_kernel", (t, R, str(npoly), "false", "2", "false")))
-        for ck in (True, False):                       # ZG_SCAN_TPC=4
-            opt.add(("scan_fwd_tma_kernel", (t, "0", "0", _b(ck), "4", "false")))
-        for ck in (True, False):                       # tpc2 (round-1 fallback); ZG_SCAN_TPC2_NPOLY
-            dflt.add(("scan_fwd_tpc2_kernel", (t, "0", _b(ck))))
-        for npoly in (1, 2):
-            opt.add(("scan_fwd_tpc2_kernel", (t, str(npoly), "false")))
-        for tma in (False, True):                      # ZG_SCAN_WP = 1 / 2 (and ZG_SCAN_WP_NPOLY = 1)
-            opt.add(("scan_fwd_wp_kernel", (t, "true", "false", _b(tma), "0")))
+        for ck in (True, False):
             for plain in (False, True):
-                opt.add(("scan_fwd_wp_kernel", (t, "false", _b(plain), _b(tma), "0")))
-        opt.add(("scan_fwd_wp_kernel", (t, "false", "true", "false", "1")))
-        for plain in (False, True):                    # wp2: the automatic choice's mode 3 (inference calls) ...
-            dflt.add(("scan_fwd_wp2_kernel", (t, "false", _b(plain), "false")))
-            opt.add(("scan_fwd_wp2_kernel", (t, "false", _b(plain), "true")))       # ... ZG_SCAN_WP = 4
-            dflt.add(("scan_fwd_wph_kernel", (t, "false", _b(plain))))             # wph: mode 5
-        opt.add(("scan_fwd_wp2_kernel", (t, "true", "false", "false")))             # checkpoints: ZG_SCAN_WP = 3 / 4 / 5 only
-        opt.add(("scan_fwd_wp2_kernel", (t, "true", "false", "true")))
-        opt.add(("scan_fwd_wph_kernel", (t, "true", "false")))
+                dflt.add(("scan_fwd_tma_kernel", (t, "0", _b(ck), _b(plain))))
+            for R in ("40", "48"):
+                dflt.add(("scan_fwd_tma_kernel", (t, R, _b(ck), "false")))
+            dflt.add(("scan_fwd_tpc2_kernel", (t, _b(ck))))               # tpc2 (round-1 fallback)
+        for plain in (False, True):                    # inference calls only: wp2 = the automatic choice's mode 3, wph = mode 5
+            dflt.add(("scan_fwd_wp2_kernel", (t, _b(plain))))
+            dflt.add(("scan_fwd_wph_kernel", (t, _b(plain))))
     for t in T_ALL:                                    # backward: generic (NS, constant B / C), q4 (staged or not), DET both ways
         for det in (False, True):
             for ns in (8, 16, 32, 64):
@@ -758,10 +733,10 @@ def _inventory():
                     dflt.add(("scan_bwd_kernel", (t, str(ns), _b(cb), _b(det))))
             for st in (False, True):
                 dflt.add(("scan_bwd_q4_kernel", (t, _b(st), _b(det))))
-    return dflt, opt
+    return dflt
 
 
-DEFAULT, OPT_IN = _inventory()
+DEFAULT = _inventory()
 SCAN_RE = re.compile(r"zg::(scan_(?:fwd|bwd)\w*_kernel)<(.*)>\(")
 
 
@@ -780,9 +755,9 @@ def _tool(name):
 
 
 def test_inventory_matches_library():
-    """CPU: the zg::scan_fwd* / zg::scan_bwd* kernels in the built library are exactly DEFAULT | OPT_IN (124 + 66): a new
-    instantiation fails here until this file tests it."""
-    assert len(DEFAULT) == 124 and len(OPT_IN) == 66 and not DEFAULT & OPT_IN
+    """CPU: the zg::scan_fwd* / zg::scan_bwd* kernels in the built library are exactly DEFAULT (124): a new instantiation fails
+    here until this file tests it."""
+    assert len(DEFAULT) == 124
     cuobjdump, filt = _tool("cuobjdump"), _tool("cu++filt")
     if cuobjdump is None or filt is None:
         pytest.skip("cuobjdump / cu++filt not available")
@@ -797,7 +772,7 @@ def test_inventory_matches_library():
         m = SCAN_RE.search(dem)
         if m:
             found.add((m.group(1), _template_args(m.group(2))))
-    missing, extra = sorted((DEFAULT | OPT_IN) - found), sorted(found - (DEFAULT | OPT_IN))
+    missing, extra = sorted(DEFAULT - found), sorted(found - DEFAULT)
     assert not missing and not extra, f"in the table, not in the library: {missing}\nin the library, not in the table: {extra}"
 
 
@@ -822,49 +797,3 @@ def test_matrix_launches_exactly_default():
     seen = _launched(lambda: [run_case(c, check=False) for c in CASES])
     missing, extra = sorted(DEFAULT - seen), sorted(seen - DEFAULT)
     assert not missing and not extra, f"not launched: {missing}\nlaunched but not DEFAULT: {extra}"
-
-
-# ------------------------------------------------------------------------------------------------ opt-in variants
-# Hot-path cases the switches act on: the model's call (plain) with and without checkpoints, a non-plain call (no z / reverse +
-# accumulate), the fused prologue, a misaligned D (the tpc2 kernel), and the generic dstate-16 kernel in both layouts (L 45).
-OPT_CASES = [c for c in CASES if c.N == 16 and c.batch <= 8 and (
-    (c.T in LOWP and c.dim == 128 and c.L == 64 and c.varB and c.varC and c.layout == "tok" and not c.strided and c.misalign in (None, "D"))
-    or (c.dim == 96 and c.L == 45 and c.varB and c.varC and not c.strided))]
-
-
-def _run_opt_cases(path):
-    """Every OPT_CASES entry, forward checked against fp64 (no backward: the switches are forward-only); writes the kernels it
-    launched to `path`."""
-    seen = _launched(lambda: [run_case(Case(c, bwd=False)) for c in OPT_CASES])
-    with open(path, "w") as f:
-        json.dump(sorted([k, list(a)] for k, a in seen), f)
-
-
-# the switches read once per process, grouped into as few children as possible
-CHILD_ENVS = ({"ZG_SCAN_NPOLY": "2", "ZG_SCAN_TMA_NPOLY": "1", "ZG_SCAN_TPC2_NPOLY": "1"},
-              {"ZG_SCAN_NPOLY": "3", "ZG_SCAN_TMA_NPOLY": "2", "ZG_SCAN_TPC2_NPOLY": "2"},
-              {"ZG_SCAN_NPOLY": "4", "ZG_SCAN_TPC": "4"})
-
-
-@gpu
-def test_opt_in_variants_vs_fp64(tmp_path, monkeypatch):
-    """The opt-in instantiations against the same fp64 bounds.  ZG_SCAN_WP (1..5) and ZG_SCAN_WP_NPOLY are read at each call and
-    set here; the switches read once per process run in child processes.  The union of what they launch covers OPT_IN."""
-    seen = set()
-    for wp in ("1", "2", "3", "4", "5"):
-        for wp_npoly in (("0", "1") if wp == "1" else ("0",)):
-            monkeypatch.setenv("ZG_SCAN_WP", wp)
-            monkeypatch.setenv("ZG_SCAN_WP_NPOLY", wp_npoly)
-            cases = [Case(c, bwd=False) for c in OPT_CASES if c.layout == "tok" and c.misalign is None]
-            seen |= _launched(lambda: [run_case(c) for c in cases])
-    monkeypatch.delenv("ZG_SCAN_WP")
-    monkeypatch.delenv("ZG_SCAN_WP_NPOLY")
-    tests = os.path.join(ROOT, "tests")
-    for k, env in enumerate(CHILD_ENVS):
-        out = tmp_path / f"child{k}.json"
-        code = f"import sys; sys.path.insert(0, {tests!r}); sys.path.insert(0, {ROOT!r}); import test_gpu_scan_kernels as t; t._run_opt_cases({str(out)!r})"
-        r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd=ROOT, env=dict(os.environ, **env), timeout=1200)
-        assert r.returncode == 0, f"child {env}:\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}"
-        seen |= {(k_, tuple(a)) for k_, a in json.load(open(out))}
-    missing, extra = sorted(OPT_IN - seen), sorted(seen - OPT_IN - DEFAULT)
-    assert not missing and not extra, f"opt-in not launched: {missing}\nlaunched, in neither table: {extra}"

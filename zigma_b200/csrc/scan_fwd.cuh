@@ -26,9 +26,6 @@ namespace zg {
 
 constexpr int SCAN_CH = 64;      // channels (= threads) per CTA
 constexpr int SCAN_TL = 16;      // time steps per pipeline stage
-#ifndef ZG_SCAN_NPOLY_DEFAULT
-#define ZG_SCAN_NPOLY_DEFAULT 0
-#endif
 constexpr int SCAN_SB = 4;       // time steps processed together by the packed inner loop
 // The register file is split per SMSP (16384 x 32-bit each): 5 warps per SMSP need <= 96 registers per
 // thread.  At bs=64, E=1280 the grid has 2560 warps = 17.3 per SM; with 4 warps per SMSP (100+
@@ -62,8 +59,7 @@ __device__ __forceinline__ void copy_chunk(T *sdst, const T *gsrc, int nvalid) {
     }
 }
 
-// NPOLY: how many of the NS/2 state PAIRS take their exp2 from the FMA-pipe polynomial instead of MUFU
-template <typename T, int NS, bool SEQ, bool CONSTBC, int NPOLY>
+template <typename T, int NS, bool SEQ, bool CONSTBC>
 __global__ void __launch_bounds__(SCAN_CH, (NS <= 16 && !CONSTBC) ? SCAN_MIN_CTAS : 1) scan_fwd_kernel(const zg_scan_params p) {
     using SM = ScanSmem<T, SEQ>;
     constexpr int VEC = SM::VEC;
@@ -224,7 +220,6 @@ __global__ void __launch_bounds__(SCAN_CH, (NS <= 16 && !CONSTBC) ? SCAN_MIN_CTA
     // SB steps are independent, so their MUFU latency overlaps; the state update is 4 packed
     // instructions + 2 exp2 per state PAIR and step:
     //     x = dl * A'      a = 2^x      h = a * h + (dl*u) * B      y += C * h
-    // The first NPOLY pairs take 2^x from the FMA-pipe polynomial (zg_ex2_poly2), the rest from MUFU.
     auto block = [&](int t0, const float (&uu)[SB], const float (&dd)[SB], const float (&zz)[SB], float (&y)[SB]) {
         zg_f2 dl2[SB], du2[SB], y2[SB];
 #pragma unroll
@@ -246,7 +241,7 @@ __global__ void __launch_bounds__(SCAN_CH, (NS <= 16 && !CONSTBC) ? SCAN_MIN_CTA
                     if (!varC) Cv = make_float2(Cc[2 * q], Cc[2 * q + 1]);
                 }
                 const zg_f2 x = zg_mul2(dl2[i], Al2p[q]);
-                const zg_f2 a = (q < NPOLY) ? zg_ex2_poly2(x) : zg_ex2_mufu2(x);
+                const zg_f2 a = zg_ex2_mufu2(x);
                 h2[q] = zg_fma2(a, h2[q], zg_mul2(du2[i], Bv));
                 y2[i] = zg_fma2(Cv, h2[q], y2[i]);
             }
@@ -412,13 +407,13 @@ __global__ void __launch_bounds__(SCAN_CH, (NS <= 16 && !CONSTBC) ? SCAN_MIN_CTA
     if (active && p.last_state) store_state(p.last_state + ((int64_t)b * E + e) * N);
 }
 
-template <typename T, int NS, bool SEQ, bool CONSTBC, int NPOLY = 0>
+template <typename T, int NS, bool SEQ, bool CONSTBC>
 int launch_scan_fwd(const zg_scan_params &p, cudaStream_t stream) {
     using SM = ScanSmem<T, SEQ>;
     const int per_group = p.dim / p.ngroups;
     const int tiles = p.ngroups * ((per_group + SCAN_CH - 1) / SCAN_CH);
     const int smem = SM::total_bytes(NS);
-    auto kern = scan_fwd_kernel<T, NS, SEQ, CONSTBC, NPOLY>;
+    auto kern = scan_fwd_kernel<T, NS, SEQ, CONSTBC>;
     static bool attr_set = false;   // per instantiation
     if (!attr_set) {
         cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -434,31 +429,6 @@ int launch_scan_fwd(const zg_scan_params &p, cudaStream_t stream) {
     zg_count_launch();
     zg_note_scan_kernel("zg::scan_fwd_kernel (generic: one thread per channel)");
     return zg_check_launch("scan_fwd");
-}
-
-// How many state pairs use the polynomial exp2 (tuning knob; default carried over from measurements on another GPU; not re-tuned on H100
-// in DESIGN.md).  ZG_SCAN_NPOLY in the environment overrides it (read once).
-inline int scan_npoly_setting() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("ZG_SCAN_NPOLY");
-        v = e ? atoi(e) : ZG_SCAN_NPOLY_DEFAULT;
-        if (v != 0 && v != 2 && v != 3 && v != 4) v = ZG_SCAN_NPOLY_DEFAULT;
-    }
-    return v;
-}
-
-// one translation unit per I/O dtype (parallel compilation)
-template <typename T, int NS, bool SEQ> int launch_scan_fwd_npoly(const zg_scan_params &p, cudaStream_t stream) {
-    if (NS == 16) {
-        switch (scan_npoly_setting()) {
-            case 2: return launch_scan_fwd<T, NS, SEQ, false, (NS == 16 ? 2 : 0)>(p, stream);
-            case 3: return launch_scan_fwd<T, NS, SEQ, false, (NS == 16 ? 3 : 0)>(p, stream);
-            case 4: return launch_scan_fwd<T, NS, SEQ, false, (NS == 16 ? 4 : 0)>(p, stream);
-            default: break;
-        }
-    }
-    return launch_scan_fwd<T, NS, SEQ, false, 0>(p, stream);
 }
 
 // Pure part of scan_auto_choice (scan_fwd_tma.cuh; exported as zg_scan_kernel_choice so that the rule is testable without a GPU):
@@ -501,8 +471,8 @@ unsupported:
         return zg_set_error("selective_scan_fwd: OUT_REVERSE / OUT_ACCUMULATE are implemented by the hot-path kernel only (16-bit dim-contiguous, dstate 16, seqlen %% 8 == 0, dim %% 64 == 0)");
 #define ZG_SCAN_CASE(NSV)                                                                   \
     if (N <= NSV) {                                                                         \
-        if (seq) return launch_scan_fwd_npoly<T, NSV, true>(p, stream);                     \
-        return launch_scan_fwd_npoly<T, NSV, false>(p, stream);                             \
+        if (seq) return launch_scan_fwd<T, NSV, true, false>(p, stream);                    \
+        return launch_scan_fwd<T, NSV, false, false>(p, stream);                            \
     }
     if (constbc) {
         if (N <= 8) return seq ? launch_scan_fwd<T, 8, true, true>(p, stream) : launch_scan_fwd<T, 8, false, true>(p, stream);

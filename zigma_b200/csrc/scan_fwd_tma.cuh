@@ -29,7 +29,7 @@
 //              the CTA's dt_proj rows (kept in shared memory), rounded to the I/O dtype like the reference's GEMM output:
 //              the (batch, dim, seqlen) delta tensor never exists in HBM and the dt_proj GEMM launch disappears.
 //   main       two threads per channel, 8 states (4 fp32x2 pairs) each: per step one LDS.64 (delta', delta' u), four
-//              LDS.128 (B, C), 4 x {pair multiply, 2 MUFU.EX2 | polynomial, pair multiply, 2 pair FMAs}, one FADD, one STS (the partial
+//              LDS.128 (B, C), 4 x {pair multiply, 2 MUFU.EX2, pair multiply, 2 pair FMAs}, one FADD, one STS (the partial
 //              y overwrites the (delta', delta' u) slot it came from).
 //   post       y = y_lo + y_hi + D u, SiLU(z) gate, bf16x2 pack, 4-byte stores.
 #pragma once
@@ -37,19 +37,6 @@
 #include <cuda.h>
 #include <string.h>
 #include <type_traits>
-
-#ifndef ZG_SCAN_EXP
-#define ZG_SCAN_EXP 0      // 1, 2: timing experiments (wrong results), see DESIGN.md
-#endif
-#ifndef ZG_SCAN_SWP
-#define ZG_SCAN_SWP 1      // hand software-pipelined recurrence loop (0: the straight loop)
-#endif
-#ifndef ZG_SCAN_WP_DEFAULT
-#define ZG_SCAN_WP_DEFAULT -1  // -1: chosen per call (scan_auto_choice); 0: CTA-wide phases (this file); 1 / 2: warp-private pipeline (scan_fwd_wp.cuh), cp.async / TMA staging; 3 / 4: two channels per lane (scan_fwd_wp2.cuh); 5: mixed CTAs (scan_fwd_wph.cuh)
-#endif
-#ifndef ZG_SCAN_TMA_NPOLY_DEFAULT
-#define ZG_SCAN_TMA_NPOLY_DEFAULT 0
-#endif
 
 namespace zg {
 
@@ -59,7 +46,7 @@ constexpr int PT_F32ROW = 576;        // pitch of one step of the fp32 pair tile
 
 __host__ __device__ constexpr int pt_pitch16(int bytes) { return ((bytes / 16) | 1) * 16; }   // odd number of 16-byte units
 
-template <int R, int TPC = 2> struct PtLayout {           // R = dt_rank of the fused prologue, 0 = delta comes from HBM; TPC = threads per channel
+template <int R> struct PtLayout {                       // R = dt_rank of the fused prologue, 0 = delta comes from HBM
     static constexpr bool FUSE = R > 0;
     static constexpr int NSTAGE = 3;
     static constexpr int NSWZ = FUSE ? 2 : 3;                         // swizzled 8 x 128 B tiles per stage: u, z (, delta)
@@ -72,30 +59,10 @@ template <int R, int TPC = 2> struct PtLayout {           // R = dt_rank of the 
     static constexpr int XSTAGE = FUSE ? ((PT_TL * XBYTES + 127) / 128) * 128 : PT_TL * 64;
     static constexpr int DDU_OFF = X_OFF + NSTAGE * XSTAGE;           // (delta', delta' u) fp32 pairs; the partial y overwrite them
     static constexpr int BCF_OFF = DDU_OFF + PT_TL * PT_F32ROW;       // fp32 [step][B0..15 C0..15]
-    static constexpr int YROW = 64 * 4 * TPC + 64;                    // TPC > 2: separate partial-y tile, TPC floats per channel and step
-    static constexpr int Y_OFF = BCF_OFF + PT_TL * 32 * 4;
-    static constexpr int W_OFF = Y_OFF + (TPC > 2 ? PT_TL * YROW : 0);
+    static constexpr int W_OFF = BCF_OFF + PT_TL * 32 * 4;
     static constexpr int BAR_OFF = W_OFF + (FUSE ? PT_CH * WROW : 0);
     static constexpr int TOTAL = BAR_OFF + NSTAGE * 8;
 };
-
-// 2^x for x <= 0 (two lanes) on the FMA / ALU pipes: see zg_ex2_poly2; only the underflow side needs a clamp here
-__device__ __forceinline__ zg_f2 zg_ex2_poly2_neg(zg_f2 x) {
-    x.x = fmaxf(x.x, -126.f);
-    x.y = fmaxf(x.y, -126.f);
-    const zg_f2 r = zg_add2(x, zg_splat2(12582912.f));
-    const zg_f2 xi = zg_add2(r, zg_splat2(-12582912.f));
-    const zg_f2 f = zg_add2(x, zg_mul2(xi, zg_splat2(-1.f)));
-    zg_f2 p = zg_splat2(0.001327647129073739f);
-    p = zg_fma2(p, f, zg_splat2(0.009675540961325169f));
-    p = zg_fma2(p, f, zg_splat2(0.05550713092088699f));
-    p = zg_fma2(p, f, zg_splat2(0.24022120237350464f));
-    p = zg_fma2(p, f, zg_splat2(0.6931469440460205f));
-    p = zg_fma2(p, f, zg_splat2(1.0000001192092896f));
-    p.x = __int_as_float(__float_as_int(p.x) + (__float_as_int(r.x) << 23));
-    p.y = __int_as_float(__float_as_int(p.y) + (__float_as_int(r.y) << 23));
-    return p;
-}
 
 template <typename T> __device__ __forceinline__ float2 pt_unpack2(uint32_t v);
 template <> __device__ __forceinline__ float2 pt_unpack2<__nv_bfloat16>(uint32_t v) {
@@ -133,32 +100,11 @@ __device__ __forceinline__ float2 pt_softplus20_2(float2 x) {
     r.y = (x.y > 20.f) ? x.y : r.y;
     return r;
 }
-// 1 / d for d in [1, 2^126] on the FMA pipe: integer-subtraction seed (relative error < 12.5 %) and three Newton steps in the
-// residual form r += r (1 - d r); maximum relative error 6.8e-8 over the range (MUFU.RCP: 1.2e-7).
-__device__ __forceinline__ float2 pt_rcp2_fma(float2 d) {
-    float2 r = make_float2(__int_as_float(0x7EF311C7 - __float_as_int(d.x)), __int_as_float(0x7EF311C7 - __float_as_int(d.y)));
-    const float2 nd = make_float2(-d.x, -d.y), one = zg_splat2(1.f);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) r = zg_fma2(r, zg_fma2(nd, r, one), r);
-    return r;
-}
-// SiLU of a channel pair.  ZG_SCAN_RCP_FMA: the reciprocal of the sigmoid on the FMA pipe instead of MUFU.RCP -- the scan kernels
-// are bound by the MUFU pipe (20 per (b, e, l), one of them this reciprocal) and have issue slots to spare.  The exponent is
-// clamped so that 1 + 2^t stays finite (z < -87: silu(z) ~ -1e-36 instead of -0).
-#ifndef ZG_SCAN_RCP_FMA
-#define ZG_SCAN_RCP_FMA 0
-#endif
+// SiLU of a channel pair
 __device__ __forceinline__ float2 pt_silu2(float2 z) {
-    float2 t = zg_mul2(z, zg_splat2(-ZG_LOG2E));
-#if ZG_SCAN_RCP_FMA
-    t.x = fminf(t.x, 126.f);
-    t.y = fminf(t.y, 126.f);
-    const float2 d = zg_add2(make_float2(zg_ex2(t.x), zg_ex2(t.y)), zg_splat2(1.f));
-    return zg_mul2(z, pt_rcp2_fma(d));
-#else
+    const float2 t = zg_mul2(z, zg_splat2(-ZG_LOG2E));
     const float2 d = zg_add2(make_float2(zg_ex2(t.x), zg_ex2(t.y)), zg_splat2(1.f));
     return zg_mul2(z, make_float2(zg_rcp(d.x), zg_rcp(d.y)));
-#endif
 }
 
 __device__ __forceinline__ void pt_ldmatrix_x4(uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3, uint32_t saddr) {
@@ -194,91 +140,52 @@ template <typename T> __device__ __forceinline__ void pt_mma_k8(float &d0, float
     }
 }
 
-// one stage (8 steps) of the recurrence for this thread's 16 / TPC states (NPAIR fp32x2 pairs); NP of the pairs use the FMA-pipe exp2.
-// ddu_c: this channel's (delta', delta' u) pairs, one per step.  ypart: where this thread's partial y of step t goes (+ t * ypitch):
-// with two threads per channel the two halves overwrite the pair they were computed from, else a separate tile.
-// Software-pipelined by hand (ZG_SCAN_SWP, default on): ptxas emits the unrolled steps strictly one after the other
-// (LDS -> multiplies -> 8 MUFU -> FMA chain -> STS, ~140 cycles of dependent latency per step and warp), so the decay factors
-// exp2(delta' A) of step t + 1 -- which depend on nothing but (delta', A) -- are issued BEFORE the FMA part of step t.
-template <int NP, int TPC, int PITCH = PT_F32ROW>
-__device__ __forceinline__ void pt_main_stage(const unsigned char *__restrict__ ddu_c, const float *__restrict__ bcf_p, unsigned char *__restrict__ ypart, int ypitch,
-                                              zg_f2 (&h2)[8 / TPC], const zg_f2 (&Al2p)[8 / TPC], bool store = true, int sync_step = -1, int bar_threads = 0) {
-    constexpr int NPAIR = 8 / TPC, NQ = 4 / TPC;           // state pairs per thread; float4 loads of B (and of C) per step
-    auto decay = [&](float dlx, zg_f2 (&a)[NPAIR]) {
+// one stage (8 steps) of the recurrence for this thread's 8 states (4 fp32x2 pairs).  ddu_c: this channel's (delta', delta' u) pairs,
+// one per step, pitch PITCH.  ypart: where this thread's partial y of step t goes (+ t * PITCH): the two threads of a channel overwrite
+// the pair they were computed from.
+// Software-pipelined by hand: ptxas emits the unrolled steps strictly one after the other (LDS -> multiplies -> 8 MUFU -> FMA chain
+// -> STS, ~140 cycles of dependent latency per step and warp), so the decay factors exp2(delta' A) of step t + 1 -- which depend on
+// nothing but (delta', A) -- are issued BEFORE the FMA part of step t.
+template <int PITCH = PT_F32ROW>
+__device__ __forceinline__ void pt_main_stage(const unsigned char *__restrict__ ddu_c, const float *__restrict__ bcf_p, unsigned char *__restrict__ ypart,
+                                              zg_f2 (&h2)[4], const zg_f2 (&Al2p)[4]) {
+    auto decay = [&](float dlx, zg_f2 (&a)[4]) {
         const zg_f2 dl = zg_splat2(dlx);
 #pragma unroll
-        for (int q = 0; q < NPAIR; ++q) {
-            const zg_f2 x = zg_mul2(dl, Al2p[q]);
-#if ZG_SCAN_EXP == 5
-            a[q] = zg_add2(x, zg_splat2(1.f));              // experiment: everything but the exponentials
-#else
-            a[q] = (q < NP) ? zg_ex2_poly2_neg(x) : zg_ex2_mufu2(x);
-#endif
-        }
+        for (int q = 0; q < 4; ++q) a[q] = zg_ex2_mufu2(zg_mul2(dl, Al2p[q]));
     };
-#if ZG_SCAN_SWP
-    zg_f2 a_cur[NPAIR];
+    zg_f2 a_cur[4];
     float2 dd = *reinterpret_cast<const float2 *>(ddu_c);
     decay(dd.x, a_cur);
 #pragma unroll
     for (int t = 0; t < PT_TL; ++t) {
         const float4 *bc = reinterpret_cast<const float4 *>(bcf_p + t * 32);
-        zg_f2 Bp[NPAIR], Cp[NPAIR];
+        zg_f2 Bp[4], Cp[4];
 #pragma unroll
-        for (int k = 0; k < NQ; ++k) {
+        for (int k = 0; k < 2; ++k) {
             const float4 Bk = bc[k], Ck = bc[4 + k];
             Bp[2 * k] = make_float2(Bk.x, Bk.y); Bp[2 * k + 1] = make_float2(Bk.z, Bk.w);
             Cp[2 * k] = make_float2(Ck.x, Ck.y); Cp[2 * k + 1] = make_float2(Ck.z, Ck.w);
         }
         const zg_f2 du = zg_splat2(dd.y);
-        zg_f2 a_nxt[NPAIR];
+        zg_f2 a_nxt[4];
         if (t + 1 < PT_TL) {                               // next step's pair and decays: in flight during this step's FMAs
             dd = *reinterpret_cast<const float2 *>(ddu_c + (t + 1) * PITCH);
             decay(dd.x, a_nxt);
         }
         zg_f2 y2 = zg_splat2(0.f);
 #pragma unroll
-        for (int q = 0; q < NPAIR; ++q) {
+        for (int q = 0; q < 4; ++q) {
             h2[q] = zg_fma2(a_cur[q], h2[q], zg_mul2(du, Bp[q]));
             y2 = zg_fma2(Cp[q], h2[q], y2);
         }
-        *reinterpret_cast<float *>(ypart + t * ypitch) = y2.x + y2.y;
-        // staggered fairness barrier of the warp-private kernels (scan_fwd_wp.cuh): warp w of a CTA arrives after step w % 8
-        if (t == sync_step) asm volatile("bar.sync 1, %0;" ::"r"(bar_threads) : "memory");
+        // (both threads of the channel have read the pair -- one converged LDS -- before either overwrites its half)
+        *reinterpret_cast<float *>(ypart + t * PITCH) = y2.x + y2.y;
         if (t + 1 < PT_TL) {
 #pragma unroll
-            for (int q = 0; q < NPAIR; ++q) a_cur[q] = a_nxt[q];
+            for (int q = 0; q < 4; ++q) a_cur[q] = a_nxt[q];
         }
     }
-#else
-#pragma unroll
-    for (int t = 0; t < PT_TL; ++t) {
-        const float2 dd = *reinterpret_cast<const float2 *>(ddu_c + t * PITCH);      // (delta', delta' * u)
-        const float4 *bc = reinterpret_cast<const float4 *>(bcf_p + t * 32);
-        zg_f2 Bp[NPAIR], Cp[NPAIR];
-#pragma unroll
-        for (int k = 0; k < NQ; ++k) {
-            const float4 Bk = bc[k], Ck = bc[4 + k];
-            Bp[2 * k] = make_float2(Bk.x, Bk.y); Bp[2 * k + 1] = make_float2(Bk.z, Bk.w);
-            Cp[2 * k] = make_float2(Ck.x, Ck.y); Cp[2 * k + 1] = make_float2(Ck.z, Ck.w);
-        }
-        const zg_f2 du = zg_splat2(dd.y);
-        zg_f2 a[NPAIR];
-        decay(dd.x, a);
-        zg_f2 y2 = zg_splat2(0.f);
-#pragma unroll
-        for (int q = 0; q < NPAIR; ++q) {
-            h2[q] = zg_fma2(a[q], h2[q], zg_mul2(du, Bp[q]));
-            y2 = zg_fma2(Cp[q], h2[q], y2);
-        }
-        // (TPC == 2: both threads of the channel have read the pair -- one converged LDS -- before either overwrites its half)
-#if ZG_SCAN_EXP == 3
-        if (store) *reinterpret_cast<float *>(ypart + t * ypitch) = y2.x + y2.y;
-#else
-        *reinterpret_cast<float *>(ypart + t * ypitch) = y2.x + y2.y;
-#endif
-    }
-#endif
 }
 
 struct PtMaps { CUtensorMap u, d, z; };    // (channels | x_dbl columns, seqlen, batch) tensor tiles of u, delta | x_dbl, z
@@ -293,18 +200,15 @@ __device__ __forceinline__ void pt_cp_async_arrive(uint64_t *bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(zg_smem_u32(bar)) : "memory");
 }
 
-// TPC threads per channel: 2 (16 / 2 = 8 states per thread, 128-thread CTAs, 9 CTAs / SM) is the product mapping; 4 (4 states per
-// thread, 256-thread CTAs: twice the warps for the same instructions per (b, e, l)) is an experiment for under-occupied shapes
-// (ZG_SCAN_TPC=4) that measured slower, see pt_launch_variant.
+// Two threads per channel, 8 states each: 128-thread CTAs, 9 CTAs / SM.
 // PLAIN: the sampling / training call as the model makes it -- z gate present, softplus on, output in place and in order
 // (no OUT_REVERSE / OUT_ACCUMULATE) -- with those choices compiled in: no uniform branches and no predicated-off accumulate code
 // in the stage loop (post + pre 187 instead of ~250 SASS instructions; 0.502 vs 0.518 ms at config 2, same box, ZG_SCAN_PLAIN=0).
-template <typename T, int R, int NPOLY, bool CKPT, int TPC = 2, bool PLAIN = false>
-__global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kernel(const zg_scan_params p, const __grid_constant__ PtMaps maps) {
+template <typename T, int R, bool CKPT, bool PLAIN = false>
+__global__ void __launch_bounds__(128, 9) scan_fwd_tma_kernel(const zg_scan_params p, const __grid_constant__ PtMaps maps) {
     static_assert(sizeof(T) == 2, "16-bit I/O only");
-    static_assert(TPC == 2 || (TPC == 4 && R == 0 && NPOLY == 0), "four threads per channel: unfused, MUFU-only instantiation");
-    using LY = PtLayout<R, TPC>;
-    constexpr int PT_THREADS = 64 * TPC, NPAIR = 8 / TPC, NITEM = 4 / TPC;      // (step, channel pair) items per thread in pre / post
+    using LY = PtLayout<R>;
+    constexpr int PT_THREADS = 128, NPAIR = 4, NITEM = 2;      // (step, channel pair) items per thread in pre / post
     constexpr bool FUSE = LY::FUSE;
     constexpr int NSTAGE = LY::NSTAGE, TL = PT_TL, CH = PT_CH, TILE = LY::TILE;
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -313,7 +217,7 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + LY::BAR_OFF);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int part = tid % TPC;                                     // which 16 / TPC states of the channel
+    const int part = tid % 2;                                       // which 8 states of the channel
     const int E = p.dim, L = p.seqlen;
     const int per_group = E / p.ngroups;
     const int tiles_per_group = per_group / CH;
@@ -322,7 +226,7 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     const int tile = blockIdx.x % tiles;
     const int g = tile / tiles_per_group;
     const int e0 = g * per_group + (tile % tiles_per_group) * CH;
-    const int e = e0 + tid / TPC;                                   // main phase: this thread's channel
+    const int e = e0 + tid / 2;                                     // main phase: this thread's channel
     const bool has_z = PLAIN ? true : (p.z != nullptr);
     const bool z_gather = has_z && p.z_rowmap != nullptr;           // z rows by cp.async through the table
     const bool softplus = PLAIN ? true : ((p.flags & ZG_SCAN_DELTA_SOFTPLUS) != 0);
@@ -330,12 +234,10 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
 
     // ---- per-thread constants -----------------------------------------------------------------------------------
     zg_f2 Al2p[NPAIR], h2[NPAIR];
-    bool a_pos = false;
 #pragma unroll
     for (int k = 0; k < NPAIR; ++k) {
         const float2 a = *reinterpret_cast<const float2 *>(p.A + (int64_t)e * 16 + 2 * NPAIR * part + 2 * k);
         Al2p[k] = zg_mul2(a, zg_splat2(ZG_LOG2E));
-        a_pos = a_pos || a.x > 0.f || a.y > 0.f;
         h2[k] = zg_splat2(0.f);
     }
     // The two (step, channel pair) items a thread owns in the pre and post phases (same items in both: the post phase reads
@@ -346,7 +248,7 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     float2 Dv[NITEM], biasv[NITEM];
 #pragma unroll
     for (int k = 0; k < NITEM; ++k) {
-        const int row = FUSE ? (lane >> 2) : warp + 2 * TPC * k;          // (2 TPC warps: rows warp, warp + 4 | row warp)
+        const int row = FUSE ? (lane >> 2) : warp + 4 * k;
         const int pair = FUSE ? 8 * warp + 4 * k + (lane & 3) : lane;                  // channel pair 0..31 of the tile
         it_swz[k] = row * 128 + (((pair >> 2) ^ row) << 4) + (pair & 3) * 4;
         it_ddu[k] = row * PT_F32ROW + pair * 16;
@@ -369,8 +271,6 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
                 *reinterpret_cast<const uint4 *>(gw + (int64_t)row * p.dt_w_ld + ch * 8);
         }
     }
-    // NPOLY > 0 needs delta' A <= 0 (softplus'ed delta, non-positive A) for the one-sided clamp of the polynomial
-    const bool use_poly = NPOLY > 0 && softplus && !__syncthreads_or(a_pos);
     __syncthreads();
 
     // ---- producer: thread 0 issues the tensor tiles; threads 64..127 gather one z chunk each, 64..95 a B|C chunk ----
@@ -416,7 +316,6 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     // 16 bytes of the pair tile (y read, then (delta', delta' u) written), so they are interleaved item by item: four
     // independent MUFU chains (SiLU of two items, softplus of two items) per thread instead of two after two.
     auto bc_convert = [&](const unsigned char *xt) {      // B | C rows -> fp32 [step][B0..15 C0..15]: one 16-bit pair per thread
-        if (TPC > 2 && tid >= 128) return;
         const int t = tid >> 4, j = tid & 15;
         const uint32_t raw = FUSE ? *reinterpret_cast<const uint32_t *>(xt + t * LY::XBYTES + 2 * R + j * 4)
                                   : *reinterpret_cast<const uint32_t *>(xt + t * 64 + j * 4);
@@ -468,11 +367,7 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     };
     auto pre_item = [&](int k, float2 dl, const unsigned char *sw) {     // bias, softplus, * u -> (delta', delta' u) pairs
         dl = zg_add2(dl, biasv[k]);
-#if ZG_SCAN_EXP == 1
-        if (softplus) dl = zg_mul2(dl, dl);
-#else
         if (softplus) dl = pt_softplus20_2(dl);
-#endif
         const float2 du = zg_mul2(dl, pt_unpack2<T>(*reinterpret_cast<const uint32_t *>(sw + it_swz[k])));
         float2 *dst = reinterpret_cast<float2 *>(ddu + it_ddu[k]);
         dst[0] = make_float2(dl.x, du.x);
@@ -482,27 +377,16 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     const bool out_rev = PLAIN ? false : ((p.flags & ZG_SCAN_OUT_REVERSE) != 0), out_acc = PLAIN ? false : ((p.flags & ZG_SCAN_OUT_ACCUMULATE) != 0);
     const int64_t out_row = out_rev ? -p.out_sl : p.out_sl;
     const int r0 = FUSE ? (lane >> 2) : warp;               // the thread's first row of a stage
-    const int64_t out_step = FUSE ? 8 : 4 * out_row;      // element distance between the thread's two output pairs (TPC == 2)
+    const int64_t out_step = FUSE ? 8 : 4 * out_row;      // element distance between the thread's two output pairs
     T *gout = reinterpret_cast<T *>(p.out) + (int64_t)b * p.out_sb + (int64_t)(out_rev ? L - 1 - r0 : r0) * p.out_sl + e0 +
               (FUSE ? 16 * warp + 2 * (lane & 3) : 2 * lane);
     const int64_t out_stage = (int64_t)TL * out_row;
     auto post_item = [&](int k, const unsigned char *sw) {               // y = y_lo + y_hi + D u, SiLU(z) gate, store
-        float2 ysum;
-        if constexpr (TPC == 2) {
-            const float4 yy = *reinterpret_cast<const float4 *>(ddu + it_ddu[k]);   // (lo, hi) halves of 2 channels
-            ysum = zg_add2(make_float2(yy.x, yy.z), make_float2(yy.y, yy.w));
-        } else {                                          // 4 partial sums per channel in the separate y tile
-            const float4 *yp = reinterpret_cast<const float4 *>(smem + LY::Y_OFF + (it_ddu[k] / PT_F32ROW) * LY::YROW + ((it_ddu[k] % PT_F32ROW) / 16) * 32);
-            const float4 a4 = yp[0], b4 = yp[1];
-            ysum = make_float2((a4.x + a4.y) + (a4.z + a4.w), (b4.x + b4.y) + (b4.z + b4.w));
-        }
+        const float4 yy = *reinterpret_cast<const float4 *>(ddu + it_ddu[k]);   // (lo, hi) halves of 2 channels
+        const float2 ysum = zg_add2(make_float2(yy.x, yy.z), make_float2(yy.y, yy.w));
         const float2 u2 = pt_unpack2<T>(*reinterpret_cast<const uint32_t *>(sw + it_swz[k]));
         float2 y = zg_fma2(Dv[k], u2, ysum);
-#if ZG_SCAN_EXP == 1
-        if (has_z) y = zg_mul2(y, pt_unpack2<T>(*reinterpret_cast<const uint32_t *>(sw + TILE + it_swz[k])));
-#else
         if (has_z) y = zg_mul2(y, pt_silu2(pt_unpack2<T>(*reinterpret_cast<const uint32_t *>(sw + TILE + it_swz[k]))));
-#endif
         uint32_t *dst = reinterpret_cast<uint32_t *>(gout + (k ? out_step : 0));
         if (out_acc) {      // out = round(out + round(y)): the eager sum of two I/O-dtype tensors (mamba_simple.py:337)
             const float2 prev = pt_unpack2<T>(*dst), yr = pt_unpack2<T>(pt_pack2<T>(y.x, y.y));
@@ -512,10 +396,9 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     };
 
     // ---- the pipeline ------------------------------------------------------------------------------------------------
-    const unsigned char *ddu_c = ddu + (tid / TPC) * 8;
+    const unsigned char *ddu_c = ddu + (tid / 2) * 8;
     const float *bcf_p = bcf + 2 * NPAIR * part;
-    unsigned char *ypart = TPC == 2 ? ddu + (tid / TPC) * 8 + part * 4 : smem + LY::Y_OFF + (tid / TPC) * 16 + part * 4;
-    constexpr int ypitch = TPC == 2 ? PT_F32ROW : LY::YROW;
+    unsigned char *ypart = ddu + (tid / 2) * 8 + part * 4;
     {   // stage 0: pre only
         const unsigned char *sw = smem + LY::SWZ_OFF, *xt = smem + LY::X_OFF;
         zg_mbar_wait(&full[0], 0);
@@ -529,8 +412,7 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
     int slot = 0, nslot = 1;
     uint32_t npar = 0;                                       // phase parity of the next stage's slot
     for (int s = 0; s < nstages; ++s) {
-        if (NPOLY > 0 && use_poly) pt_main_stage<NPOLY, TPC>(ddu_c, bcf_p, ypart, ypitch, h2, Al2p);
-        else pt_main_stage<0, TPC>(ddu_c, bcf_p, ypart, ypitch, h2, Al2p, s == nstages - 1);
+        pt_main_stage(ddu_c, bcf_p, ypart, h2, Al2p);
         if constexpr (CKPT) {       // recompute seeds of the backward: state after every 8 steps, (batch, n_ckpt, dim, dstate)
             float4 *dst = reinterpret_cast<float4 *>(p.ckpt + (((int64_t)b * (L >> 3) + s) * E + e) * 16 + 2 * NPAIR * part);
 #pragma unroll
@@ -539,9 +421,6 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
         const unsigned char *sw = smem + LY::SWZ_OFF + slot * LY::NSWZ * TILE;
         const unsigned char *swn = smem + LY::SWZ_OFF + nslot * LY::NSWZ * TILE;
         const unsigned char *xtn = smem + LY::X_OFF + nslot * LY::XSTAGE;
-#if ZG_SCAN_EXP == 2 || ZG_SCAN_EXP == 3
-        if (s == nstages - 1) { for (int k = 0; k < NITEM; ++k) post_item(k, sw); }   // experiment: the recurrence alone
-#else
         __syncthreads();            // y complete; B/C tile free
         if (s + 1 < nstages) {      // post(s) interleaved with pre(s + 1)
             zg_mbar_wait(&full[nslot], npar);
@@ -557,7 +436,6 @@ __global__ void __launch_bounds__(64 * TPC, TPC == 2 ? 9 : 6) scan_fwd_tma_kerne
         gout += out_stage;
         __syncthreads();            // raw slot of stage s free; tiles of stage s + 1 complete
         issue_stage(s + NSTAGE, slot);
-#endif
         slot = nslot;
         if (++nslot == NSTAGE) { nslot = 0; npar ^= 1; }
     }
@@ -604,13 +482,13 @@ inline int pt_make_map(CUtensorMap *m, const void *base, int64_t cols, int64_t s
     return 0;
 }
 
-template <typename T, int R, int NPOLY, bool CKPT, int TPC = 2, bool PLAIN = false> int pt_launch(const zg_scan_params &p, cudaStream_t stream) {
-    if constexpr (!PLAIN && R == 0 && TPC == 2) {     // the model's own call: the specialised instantiation (ZG_SCAN_PLAIN=0: A/B timing)
+template <typename T, int R, bool CKPT, bool PLAIN = false> int pt_launch(const zg_scan_params &p, cudaStream_t stream) {
+    if constexpr (!PLAIN && R == 0) {     // the model's own call: the specialised instantiation (ZG_SCAN_PLAIN=0: A/B timing)
         static const bool plain_ok = [] { const char *e = getenv("ZG_SCAN_PLAIN"); return !(e && e[0] == '0'); }();
         if (plain_ok && p.z && (p.flags & ZG_SCAN_DELTA_SOFTPLUS) && !(p.flags & (ZG_SCAN_OUT_REVERSE | ZG_SCAN_OUT_ACCUMULATE)))
-            return pt_launch<T, R, NPOLY, CKPT, TPC, true>(p, stream);
+            return pt_launch<T, R, CKPT, true>(p, stream);
     }
-    using LY = PtLayout<R, TPC>;
+    using LY = PtLayout<R>;
     PtMaps maps;
     memset(&maps, 0, sizeof(maps));
     int rc = pt_make_map<T>(&maps.u, p.u, p.dim, p.seqlen, p.batch, p.u_sl, p.u_sb, PT_CH, true);
@@ -618,7 +496,7 @@ template <typename T, int R, int NPOLY, bool CKPT, int TPC = 2, bool PLAIN = fal
                         : pt_make_map<T>(&maps.d, p.delta, p.dim, p.seqlen, p.batch, p.delta_sl, p.delta_sb, PT_CH, true);
     if (!rc && p.z && !p.z_rowmap) rc = pt_make_map<T>(&maps.z, p.z, p.dim, p.seqlen, p.batch, p.z_sl, p.z_sb, PT_CH, true);
     if (rc) return rc;
-    auto kern = scan_fwd_tma_kernel<T, R, NPOLY, CKPT, TPC, PLAIN>;
+    auto kern = scan_fwd_tma_kernel<T, R, CKPT, PLAIN>;
     static bool attr_dev[64] = {};      // per instantiation and device
     int dev = 0;
     cudaGetDevice(&dev);
@@ -629,42 +507,28 @@ template <typename T, int R, int NPOLY, bool CKPT, int TPC = 2, bool PLAIN = fal
         attr_dev[dev & 63] = true;
     }
     const long long nblk = (long long)(p.dim / PT_CH) * p.batch;
-    kern<<<(unsigned)nblk, 64 * TPC, LY::TOTAL, stream>>>(p, maps);
+    kern<<<(unsigned)nblk, 128, LY::TOTAL, stream>>>(p, maps);
     zg_count_launch();
     zg_note_scan_kernel(R > 0 ? "zg::scan_fwd_tma_kernel (CTA-wide phases, TMA tensor tiles, fused dt_proj prologue)" : "zg::scan_fwd_tma_kernel (CTA-wide phases, TMA tensor tiles)");
     return zg_check_launch("scan_fwd(tma)");
 }
 
 template <typename T, int R> int pt_launch_variant(const zg_scan_params &p, cudaStream_t stream) {
-    static int npoly = -1;
-    if (npoly < 0) { npoly = pt_env_int("ZG_SCAN_TMA_NPOLY", ZG_SCAN_TMA_NPOLY_DEFAULT); if (npoly < 0 || npoly > 2) npoly = 0; }
-    if constexpr (R == 0) {
-        // ZG_SCAN_TPC=4: four threads per channel (twice the warps for the same work).  Opt-in only: measured SLOWER than two at
-        // every under-occupied shape it was meant for (bs 32, L 4096, E 1536: 1.72 vs 1.46 ms; bs 16, L 1024, E 1280: 0.249 vs
-        // 0.224 ms) -- eight warps per barrier cost more than the extra warps hide -- and a batch-size dependent choice would
-        // make results depend on the batch split (the partial sums of y associate differently).
-        static int tpc_env = -1;
-        if (tpc_env < 0) tpc_env = pt_env_int("ZG_SCAN_TPC", 2);
-        if (tpc_env == 4) return p.ckpt ? pt_launch<T, 0, 0, true, 4>(p, stream) : pt_launch<T, 0, 0, false, 4>(p, stream);
-    }
-    if (p.ckpt) return pt_launch<T, R, 0, true>(p, stream);        // training forward (writes the recompute seeds)
-    if (npoly == 1) return pt_launch<T, R, 1, false>(p, stream);
-    if (npoly == 2) return pt_launch<T, R, 2, false>(p, stream);
-    return pt_launch<T, R, 0, false>(p, stream);
+    return p.ckpt ? pt_launch<T, R, true>(p, stream)         // training forward (writes the recompute seeds)
+                  : pt_launch<T, R, false>(p, stream);
 }
 
-// warp-private pipeline (scan_fwd_wp.cuh), compiled in its own translation units
-int scan_fwd_wp_bf16(const zg_scan_params &p, cudaStream_t stream, int mode);
-int scan_fwd_wp_f16(const zg_scan_params &p, cudaStream_t stream, int mode);
-int scan_fwd_wp2_bf16(const zg_scan_params &p, cudaStream_t stream, int mode);     // two channels per lane (scan_fwd_wp2.cuh)
-int scan_fwd_wp2_f16(const zg_scan_params &p, cudaStream_t stream, int mode);
-int scan_fwd_wph_bf16(const zg_scan_params &p, cudaStream_t stream, int nd, int ns);   // mixed 32- / 16-channel warps (scan_fwd_wph.cuh)
+// the warp-private pipelines, compiled in their own translation units: 32 channels per warp (scan_fwd_wp2.cuh), mixed 32- / 16-channel
+// warps (scan_fwd_wph.cuh)
+int scan_fwd_wp2_bf16(const zg_scan_params &p, cudaStream_t stream);
+int scan_fwd_wp2_f16(const zg_scan_params &p, cudaStream_t stream);
+int scan_fwd_wph_bf16(const zg_scan_params &p, cudaStream_t stream, int nd, int ns);
 int scan_fwd_wph_f16(const zg_scan_params &p, cudaStream_t stream, int nd, int ns);
-template <typename T> inline int wp_dispatch(const zg_scan_params &p, cudaStream_t stream, int mode, int nd = 0, int ns = 0) {
+template <typename T> inline int wp_dispatch(const zg_scan_params &p, cudaStream_t stream, int mode, int nd, int ns) {
     if constexpr (std::is_same<T, __nv_bfloat16>::value)
-        return mode == 5 ? scan_fwd_wph_bf16(p, stream, nd, ns) : mode >= 3 ? scan_fwd_wp2_bf16(p, stream, mode) : scan_fwd_wp_bf16(p, stream, mode);
+        return mode == 5 ? scan_fwd_wph_bf16(p, stream, nd, ns) : scan_fwd_wp2_bf16(p, stream);
     else
-        return mode == 5 ? scan_fwd_wph_f16(p, stream, nd, ns) : mode >= 3 ? scan_fwd_wp2_f16(p, stream, mode) : scan_fwd_wp_f16(p, stream, mode);
+        return mode == 5 ? scan_fwd_wph_f16(p, stream, nd, ns) : scan_fwd_wp2_f16(p, stream);
 }
 
 // Which hot-path kernel runs a call (ZG_SCAN_WP unset).  All of them compute the same bits; what differs is how the work
@@ -719,15 +583,12 @@ template <typename T> int try_launch_scan_fwd_tma(const zg_scan_params &p, cudaS
     if ((long long)(p.dim / PT_CH) * p.batch > 0x7fffffffLL) return decline("grid too large");
     if (p.z_batch_inner > 0 && (!p.z || !p.z_rowmap || p.z_sbi % 8 != 0)) return decline("z_batch_inner needs z with a z_rowmap and 16-byte aligned rows");
     if (!fuse) {
-        // ZG_SCAN_WP: the warp-private pipelines: 1 / 2 = scan_fwd_wp.cuh (one channel per lane; cp.async staging / TMA tiles for
-        // u and delta), 3 / 4 = scan_fwd_wp2.cuh (two channels per lane; cp.async / TMA), 5 = scan_fwd_wph.cuh (mixed warps), 0 = this file's kernel
-        // (read at every call, unlike the other switches: the tests compare the kernels bit for bit inside one process)
-        const int wp_mode = pt_env_int("ZG_SCAN_WP", ZG_SCAN_WP_DEFAULT);
-        if (wp_mode >= 1 && wp_mode <= 5) return wp_dispatch<T>(p, stream, wp_mode);
-        if (wp_mode < 0) {
-            const ScanChoice c = scan_auto_choice(p);
-            if (c.mode) return wp_dispatch<T>(p, stream, c.mode, c.nd, c.ns);
-        }
+        // ZG_SCAN_WP overrides scan_auto_choice: 3 = scan_fwd_wp2.cuh (32-channel warps), 5 = scan_fwd_wph.cuh (mixed warps), any other
+        // value = this file's kernel, which also keeps every checkpoint call (read at every call: the tests compare the kernels bit for
+        // bit inside one process)
+        const int wp_mode = pt_env_int("ZG_SCAN_WP", -1);
+        const ScanChoice c = wp_mode < 0 ? scan_auto_choice(p) : ScanChoice{wp_mode, 0, 0};
+        if (!p.ckpt && (c.mode == 3 || c.mode == 5)) return wp_dispatch<T>(p, stream, c.mode, c.nd, c.ns);
         return pt_launch_variant<T, 0>(p, stream);
     }
     // fused prologue: B and C must be the tail of the dt_x rows (the x_dbl rows of x_proj)

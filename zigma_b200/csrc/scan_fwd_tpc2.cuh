@@ -19,12 +19,8 @@
 namespace zg {
 
 constexpr int TPC2_THREADS = 128;   // 64 channels x 2 threads
-#ifndef ZG_SCAN_TPC2_NPOLY_DEFAULT
-#define ZG_SCAN_TPC2_NPOLY_DEFAULT 0
-#endif
 
-// NPOLY of each thread's 4 state pairs take exp2 from the FMA-pipe polynomial (zg_ex2_poly2) instead of MUFU
-template <typename T, int NPOLY, bool CKPT = false>
+template <typename T, bool CKPT = false>
 __global__ void __launch_bounds__(TPC2_THREADS, 9) scan_fwd_tpc2_kernel(const zg_scan_params p) {
     static_assert(sizeof(T) == 2, "16-bit I/O only");
     constexpr int NS = 16, CH = SCAN_CH, TL = SCAN_TL, NSTAGE = 3, VEC = 8;
@@ -133,7 +129,7 @@ __global__ void __launch_bounds__(TPC2_THREADS, 9) scan_fwd_tpc2_kernel(const zg
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
                     const zg_f2 x = zg_mul2(dl2[i], Al2p[q]);
-                    const zg_f2 a = (q < NPOLY) ? zg_ex2_poly2(x) : zg_ex2_mufu2(x);
+                    const zg_f2 a = zg_ex2_mufu2(x);
                     h2[q] = zg_fma2(a, h2[q], zg_mul2(du2[i], Bp[q]));
                     y2[i] = zg_fma2(Cp[q], h2[q], y2[i]);
                 }
@@ -182,8 +178,6 @@ template <typename T> int try_launch_scan_fwd_tpc2(const zg_scan_params &p, cuda
     constexpr int smem = 3 * (3 * SCAN_TL * SCAN_CH * 2 + 2 * SCAN_TL * 16 * 2) + SCAN_TL * 32 * 4;
     const long long nblk = (long long)(p.dim / SCAN_CH) * p.batch;
     if (nblk > 0x7fffffffLL) return -1;
-    static int npoly = -1;
-    if (npoly < 0) { const char *e = getenv("ZG_SCAN_TPC2_NPOLY"); npoly = e ? atoi(e) : ZG_SCAN_TPC2_NPOLY_DEFAULT; if (npoly < 0 || npoly > 2) npoly = 0; }
     auto launch = [&](auto kern) {
         static bool attr_set = false;
         if (!attr_set) {
@@ -193,10 +187,8 @@ template <typename T> int try_launch_scan_fwd_tpc2(const zg_scan_params &p, cuda
         }
         kern<<<(unsigned)nblk, TPC2_THREADS, smem, stream>>>(p);
     };
-    if (p.ckpt) launch(scan_fwd_tpc2_kernel<T, 0, true>);          // training forward (writes the recompute seeds)
-    else if (npoly == 1) launch(scan_fwd_tpc2_kernel<T, 1>);
-    else if (npoly == 2) launch(scan_fwd_tpc2_kernel<T, 2>);
-    else launch(scan_fwd_tpc2_kernel<T, 0>);
+    if (p.ckpt) launch(scan_fwd_tpc2_kernel<T, true>);          // training forward (writes the recompute seeds)
+    else launch(scan_fwd_tpc2_kernel<T>);
     zg_count_launch();
     zg_note_scan_kernel("zg::scan_fwd_tpc2_kernel (round 1: LDGSTS ring, two threads per channel)");
     return zg_check_launch("scan_fwd(tpc2)");

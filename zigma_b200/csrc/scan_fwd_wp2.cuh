@@ -12,7 +12,7 @@
 // independent work (16 MUFU back to back per step).
 //
 // Everything else is scan_fwd_wp.cuh: a warp stages its own u / delta / z / B|C rows (8 steps per stage, 3-deep ring, one
-// mbarrier per slot, 16-byte cp.async chunks, or TMA tiles for u / delta), no block barrier.  Per channel the operations and
+// mbarrier per slot, 16-byte cp.async chunks), no block barrier.  Per channel the operations and
 // their order are those of scan_fwd_tma_kernel: results are bit-identical.
 // Semantics: selective_scan_fwd_kernel.cuh:153-171, :216-261, :280-298.
 #pragma once
@@ -41,7 +41,7 @@ struct Wp2Layout {                    // per warp
 // Software-pipelined like pt_main_stage: the 16 decay factors of step t + 1 are issued before the FMAs of step t.
 template <int PITCH>
 __device__ __forceinline__ void wp2_main_stage(const unsigned char *__restrict__ ddu_j, const float *__restrict__ bq, unsigned char *__restrict__ ypart,
-                                               zg_f2 (&h)[2][4], const zg_f2 (&Al)[2][4], int sync_step = -1, int bar_threads = 0) {
+                                               zg_f2 (&h)[2][4], const zg_f2 (&Al)[2][4]) {
     auto decay = [&](float dlx, const zg_f2 (&al)[4], zg_f2 (&a)[4]) {
         const zg_f2 dl = zg_splat2(dlx);
 #pragma unroll
@@ -78,7 +78,6 @@ __device__ __forceinline__ void wp2_main_stage(const unsigned char *__restrict__
         }
         // (both lanes of the channel pair have read the 16 bytes -- one converged LDS -- before either overwrites its half)
         *reinterpret_cast<float2 *>(ypart + t * PITCH) = make_float2(y0.x + y0.y, y1.x + y1.y);
-        if (t == sync_step) asm volatile("bar.sync 1, %0;" ::"r"(bar_threads) : "memory");      // staggered fairness barrier, see wp_body
         if (t + 1 < PT_TL) {
 #pragma unroll
             for (int q = 0; q < 4; ++q) { a0[q] = n0[q]; a1[q] = n1[q]; }
@@ -87,9 +86,8 @@ __device__ __forceinline__ void wp2_main_stage(const unsigned char *__restrict__
 }
 
 // The work of one warp: 32 channels [e0, e0 + 32) of group g of batch row b, all seqlen steps.  `smem`: the warp's Wp2Layout bytes.
-template <typename T, bool CKPT, bool PLAIN, bool TMA>
-__device__ __forceinline__ void wp2_body(const zg_scan_params &p, const PtMaps &maps, unsigned char *smem, const int lane, const int b, const int g, const int e0,
-                                         const int sync_every = 0, const int cta_warps = 0, const int sync_step = 0) {
+template <typename T, bool PLAIN>
+__device__ __forceinline__ void wp2_body(const zg_scan_params &p, unsigned char *smem, const int lane, const int b, const int g, const int e0) {
     static_assert(sizeof(T) == 2, "16-bit I/O only");
     using LY = Wp2Layout;
     constexpr int NSTAGE = LY::NSTAGE, TL = PT_TL, TILE = LY::TILE, NITEM = 4;
@@ -103,7 +101,6 @@ __device__ __forceinline__ void wp2_body(const zg_scan_params &p, const PtMaps &
     const bool has_z = PLAIN ? true : (p.z != nullptr);
     const bool softplus = PLAIN ? true : ((p.flags & ZG_SCAN_DELTA_SOFTPLUS) != 0);
     const int nstages = L / TL;
-    int sync_left = sync_every;
 
     // ---- per-thread constants -----------------------------------------------------------------------------------
     zg_f2 Al2p[2][4], h2[2][4];
@@ -123,9 +120,9 @@ __device__ __forceinline__ void wp2_body(const zg_scan_params &p, const PtMaps &
     const float2 Dv = p.D ? *reinterpret_cast<const float2 *>(p.D + e0 + 2 * pair) : make_float2(0.f, 0.f);
     const float2 biasv = p.delta_bias ? *reinterpret_cast<const float2 *>(p.delta_bias + e0 + 2 * pair) : make_float2(0.f, 0.f);
 
-    if (lane == 0) {        // full[s]: one cp.async arrival per lane and stage (+ the TMA issuer's expect_tx)
+    if (lane == 0) {        // full[s]: one cp.async arrival per lane and stage
 #pragma unroll
-        for (int s = 0; s < NSTAGE; ++s) zg_mbar_init(&full[s], TMA ? 33 : 32);
+        for (int s = 0; s < NSTAGE; ++s) zg_mbar_init(&full[s], 32);
         zg_mbar_fence_init();
     }
     __syncwarp();
@@ -149,32 +146,19 @@ __device__ __forceinline__ void wp2_body(const zg_scan_params &p, const PtMaps &
     const uint32_t z_sl2 = (uint32_t)p.z_sl * 2u;                  // byte offsets inside a batch element fit 32 bits (host check)
     const int32_t *zmap = p.z_rowmap;
     int zrow_next = has_z ? (zmap ? zmap[zr] : zr) : 0;            // (permuted) source row of the NEXT stage to issue
-    const unsigned char *u_src = nullptr, *d_src = nullptr;
-    uint32_t u_step = 0, d_step = 0;
-    if constexpr (!TMA) {
-        u_src = reinterpret_cast<const unsigned char *>(reinterpret_cast<const T *>(p.u) + (int64_t)b * p.u_sb + (int64_t)zr * p.u_sl + e0 + zj * 8);
-        d_src = reinterpret_cast<const unsigned char *>(reinterpret_cast<const T *>(p.delta) + (int64_t)b * p.delta_sb + (int64_t)zr * p.delta_sl + e0 + zj * 8);
-        u_step = (uint32_t)p.u_sl * (2u * TL);
-        d_step = (uint32_t)p.delta_sl * (2u * TL);
-    }
+    const unsigned char *u_src = reinterpret_cast<const unsigned char *>(reinterpret_cast<const T *>(p.u) + (int64_t)b * p.u_sb + (int64_t)zr * p.u_sl + e0 + zj * 8);
+    const unsigned char *d_src = reinterpret_cast<const unsigned char *>(reinterpret_cast<const T *>(p.delta) + (int64_t)b * p.delta_sb + (int64_t)zr * p.delta_sl + e0 + zj * 8);
+    const uint32_t u_step = (uint32_t)p.u_sl * (2u * TL), d_step = (uint32_t)p.delta_sl * (2u * TL);
     int s_issue = 0;                                               // stages are issued in order
     auto issue_stage = [&](int slot) {                             // all lanes
         if (s_issue >= nstages) return;
         unsigned char *raw = smem + slot * LY::RAW;
         uint64_t *bar = &full[slot];
         const int l0 = s_issue * TL;
-        if constexpr (TMA) {
-            if (lane == 0) {
-                zg_mbar_expect_tx(bar, 2 * TILE);
-                pt_tma_load_3d(raw, &maps.u, bar, e0, l0, b);
-                pt_tma_load_3d(raw + TILE, &maps.d, bar, e0, l0, b);
-            }
-        } else {
-            zg_cp_async16(raw + lane * 16, u_src);
-            zg_cp_async16(raw + TILE + lane * 16, d_src);
-            u_src += u_step;
-            d_src += d_step;
-        }
+        zg_cp_async16(raw + lane * 16, u_src);
+        zg_cp_async16(raw + TILE + lane * 16, d_src);
+        u_src += u_step;
+        d_src += d_step;
         if (has_z) {
             zg_cp_async16(raw + 2 * TILE + lane * 16, zsrc + (uint32_t)zrow_next * z_sl2);
             const int ln = l0 + TL + zr;
@@ -238,17 +222,7 @@ __device__ __forceinline__ void wp2_body(const zg_scan_params &p, const PtMaps &
     int slot = 0, nslot = 1;
     uint32_t npar = 0;                                             // phase parity of the next stage's slot
     for (int s = 0; s < nstages; ++s) {
-        int sstep = -1;
-        if (sync_every > 0 && --sync_left == 0) { sync_left = sync_every; sstep = sync_step; }
-        wp2_main_stage<LY::DDU_ROW>(ddu_j, bq, ypart, h2, Al2p, sstep, cta_warps * 32);
-        if constexpr (CKPT) {       // recompute seeds of the backward: state after every 8 steps, (batch, n_ckpt, dim, dstate)
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                float4 *dst = reinterpret_cast<float4 *>(p.ckpt + (((int64_t)b * (L >> 3) + s) * E + e + c) * 16 + 8 * part);
-                dst[0] = make_float4(h2[c][0].x, h2[c][0].y, h2[c][1].x, h2[c][1].y);
-                dst[1] = make_float4(h2[c][2].x, h2[c][2].y, h2[c][3].x, h2[c][3].y);
-            }
-        }
+        wp2_main_stage<LY::DDU_ROW>(ddu_j, bq, ypart, h2, Al2p);
         const unsigned char *raw = smem + slot * LY::RAW;
         __syncwarp();               // partial y of the stage complete; B/C tile free
         if (s + 1 < nstages) {      // post(s) interleaved with pre(s + 1): independent MUFU chains
@@ -277,8 +251,8 @@ __device__ __forceinline__ void wp2_body(const zg_scan_params &p, const PtMaps &
     }
 }
 
-template <typename T, bool CKPT, bool PLAIN, bool TMA>
-__global__ void __launch_bounds__(32 * WP2_MAX_WARPS, 2) scan_fwd_wp2_kernel(const zg_scan_params p, const __grid_constant__ PtMaps maps) {
+template <typename T, bool PLAIN>
+__global__ void __launch_bounds__(32 * WP2_MAX_WARPS, 2) scan_fwd_wp2_kernel(const zg_scan_params p) {
     extern __shared__ __align__(1024) unsigned char smem_all[];
     const int lane = threadIdx.x & 31;
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
@@ -288,29 +262,24 @@ __global__ void __launch_bounds__(32 * WP2_MAX_WARPS, 2) scan_fwd_wp2_kernel(con
     const int wu = blockIdx.x * (int)(blockDim.x >> 5) + warp;     // warps are independent: any number of them per CTA
     if (wu >= units * p.batch) return;
     const int unit = wu % units;
-    wp2_body<T, CKPT, PLAIN, TMA>(p, maps, smem_all + warp * Wp2Layout::WARP_BYTES, lane, wu / units, unit / units_per_group, unit * WP2_CH);
+    wp2_body<T, PLAIN>(p, smem_all + warp * Wp2Layout::WARP_BYTES, lane, wu / units, unit / units_per_group, unit * WP2_CH);
 }
 
-// CTA shape: see wp_pick_shape.  Half the warps of the one-channel-per-lane kernel: up to 18 per SM (112 registers) in two CTAs.
+// CTA shape.  The warps exchange nothing, so the CTA size is free; what it decides is how the SM's warp schedulers treat the warps:
+// they favour the oldest warps, which finish early, and the youngest run the tail with too few peers to keep the MUFU pipe busy.
+// When the whole problem fits one wave, the warps of an SM are therefore packed into one or two large CTAs (with two, either of them
+// alone keeps the pipe busy while the other is starved); problems of several waves keep small CTAs (finished CTAs are replaced).
+// Up to 18 warps per SM (112 registers) in two CTAs.
 inline int wp2_pick_warps(long long units, int sms) {
-    const int forced = pt_env_int("ZG_SCAN_WP_WARPS", 0);
-    if (forced >= 1 && forced <= WP2_MAX_WARPS) return forced;
     if (units > 18LL * sms) return 3;                                        // several waves: six small CTAs per SM
     const long long per_sm = (units + sms - 1) / sms;                        // warps on the fullest SM
     const int ctas_per_sm = per_sm > 4 ? 2 : 1;
     return (int)((units + (long long)sms * ctas_per_sm - 1) / ((long long)sms * ctas_per_sm));
 }
 
-template <typename T, bool CKPT, bool PLAIN, bool TMA> int wp2_launch(const zg_scan_params &p, cudaStream_t stream) {
+template <typename T, bool PLAIN> int wp2_launch(const zg_scan_params &p, cudaStream_t stream) {
     using LY = Wp2Layout;
-    PtMaps maps;
-    memset(&maps, 0, sizeof(maps));
-    if constexpr (TMA) {
-        int rc = pt_make_map<T>(&maps.u, p.u, p.dim, p.seqlen, p.batch, p.u_sl, p.u_sb, WP2_CH, false);
-        if (!rc) rc = pt_make_map<T>(&maps.d, p.delta, p.dim, p.seqlen, p.batch, p.delta_sl, p.delta_sb, WP2_CH, false);
-        if (rc) return rc;
-    }
-    auto kern = scan_fwd_wp2_kernel<T, CKPT, PLAIN, TMA>;
+    auto kern = scan_fwd_wp2_kernel<T, PLAIN>;
     static bool attr_dev[64] = {};      // per instantiation and device
     static int sms_dev[64] = {};
     int dev = 0;
@@ -325,22 +294,17 @@ template <typename T, bool CKPT, bool PLAIN, bool TMA> int wp2_launch(const zg_s
     const long long units = (long long)(p.dim / WP2_CH) * p.batch;
     const int w = wp2_pick_warps(units, sms_dev[dev & 63] > 0 ? sms_dev[dev & 63] : 132);
     const long long nblk = (units + w - 1) / w;
-    kern<<<(unsigned)nblk, 32 * w, w * LY::WARP_BYTES, stream>>>(p, maps);
+    kern<<<(unsigned)nblk, 32 * w, w * LY::WARP_BYTES, stream>>>(p);
     zg_count_launch();
-    zg_note_scan_kernel(TMA ? "zg::scan_fwd_wp2_kernel (warp-private pipeline, 32 channels per warp, TMA tiles)" : "zg::scan_fwd_wp2_kernel (warp-private pipeline, 32 channels per warp, cp.async)");
+    zg_note_scan_kernel("zg::scan_fwd_wp2_kernel (warp-private pipeline, 32 channels per warp, cp.async)");
     return zg_check_launch("scan_fwd(wp2)");
 }
 
-// mode: 3 = cp.async staging, 4 = TMA tiles for u / delta.  The caller (try_launch_scan_fwd_tma) has checked the shape class
-// (dim / groups a multiple of 64, hence of 32).
-template <typename T> int wp2_launch_variant(const zg_scan_params &p, cudaStream_t stream, int mode) {
+// mode 3.  The caller (try_launch_scan_fwd_tma) has checked the shape class (dim / groups a multiple of 64, hence of 32) and keeps
+// checkpoint calls on the CTA-wide kernel.
+template <typename T> int wp2_launch_variant(const zg_scan_params &p, cudaStream_t stream) {
     const bool plain = p.z && (p.flags & ZG_SCAN_DELTA_SOFTPLUS) && !(p.flags & (ZG_SCAN_OUT_REVERSE | ZG_SCAN_OUT_ACCUMULATE));
-    if (mode == 4) {
-        if (p.ckpt) return wp2_launch<T, true, false, true>(p, stream);
-        return plain ? wp2_launch<T, false, true, true>(p, stream) : wp2_launch<T, false, false, true>(p, stream);
-    }
-    if (p.ckpt) return wp2_launch<T, true, false, false>(p, stream);
-    return plain ? wp2_launch<T, false, true, false>(p, stream) : wp2_launch<T, false, false, false>(p, stream);
+    return plain ? wp2_launch<T, true>(p, stream) : wp2_launch<T, false>(p, stream);
 }
 
 }  // namespace zg

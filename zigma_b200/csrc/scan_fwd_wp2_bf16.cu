@@ -1,5 +1,5 @@
 // selective-scan forward, warp-private pipeline with two channels per lane, I/O dtype __nv_bfloat16 (own TU)
 #include "scan_fwd_wp2.cuh"
 namespace zg {
-int scan_fwd_wp2_bf16(const zg_scan_params &p, cudaStream_t stream, int mode) { return wp2_launch_variant<__nv_bfloat16>(p, stream, mode); }
+int scan_fwd_wp2_bf16(const zg_scan_params &p, cudaStream_t stream) { return wp2_launch_variant<__nv_bfloat16>(p, stream); }
 }  // namespace zg

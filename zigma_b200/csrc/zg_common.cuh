@@ -117,26 +117,6 @@ __device__ __forceinline__ zg_f2 zg_mul2(zg_f2 a, zg_f2 b) { return make_float2(
 __device__ __forceinline__ zg_f2 zg_add2(zg_f2 a, zg_f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 // 2^x for two lanes at once via MUFU.EX2 (2 MUFU issues)
 __device__ __forceinline__ zg_f2 zg_ex2_mufu2(zg_f2 x) { return make_float2(zg_ex2(x.x), zg_ex2(x.y)); }
-// 2^x for two lanes on the FMA/ALU pipes only (no MUFU): Cody-Waite split x = i + f, |f| <= 0.5,
-// 2^f by a degree-5 minimax polynomial (max relative error 2.3e-7 in fp32 Horner form -- the same as
-// ex2.approx's 2^-22), 2^i by adding i to the exponent field.  x is clamped to [-126, 126].
-// Used to take part of the exp load off the 16-lane/SM MUFU pipe when that pipe bounds the scan.
-__device__ __forceinline__ zg_f2 zg_ex2_poly2(zg_f2 x) {
-    x.x = fminf(fmaxf(x.x, -126.f), 126.f);
-    x.y = fminf(fmaxf(x.y, -126.f), 126.f);
-    const zg_f2 r = zg_add2(x, zg_splat2(12582912.f));              // 1.5 * 2^23: low mantissa bits = round(x)
-    const zg_f2 xi = zg_add2(r, zg_splat2(-12582912.f));
-    const zg_f2 f = zg_fma2(xi, zg_splat2(-1.f), x);
-    zg_f2 p = zg_splat2(0.001327647129073739f);
-    p = zg_fma2(p, f, zg_splat2(0.009675540961325169f));
-    p = zg_fma2(p, f, zg_splat2(0.05550713092088699f));
-    p = zg_fma2(p, f, zg_splat2(0.24022120237350464f));
-    p = zg_fma2(p, f, zg_splat2(0.6931469440460205f));
-    p = zg_fma2(p, f, zg_splat2(1.0000001192092896f));
-    p.x = __int_as_float(__float_as_int(p.x) + (__float_as_int(r.x) << 23));
-    p.y = __int_as_float(__float_as_int(p.y) + (__float_as_int(r.y) << 23));
-    return p;
-}
 
 // cp.async (LDGSTS) 16-byte copy global -> shared, L2 only (streamed data, no L1 allocation)
 __device__ __forceinline__ void zg_cp_async16(void *smem_dst, const void *gmem_src) {
