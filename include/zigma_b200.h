@@ -413,6 +413,56 @@ typedef struct {
 
 int zg_adamw_ema_step(const zg_adamw_params *p, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Text prologue of a has_text block (model_zigma.py:206-208): what lies between the mixer and the cross-attention,
+ *     hidden = x + gate * mixer_out;   q_in = modulate(norm_msa(hidden), shift_msa, scale_msa)
+ * in one pass.  Token-major (batch, seqlen, dim) contiguous rows; round() = round to `dtype` (identity for fp32), at the
+ * points the eager graph materialises a tensor:
+ *     hidden = round(x + round(gate[b] * mix[b, rowmap[l]]))          (rowmap int32[seqlen] or NULL = identity)
+ *     mean, rstd of the row of hidden in fp32:  rstd = 1 / sqrt(mean((hidden - mean)^2) + eps)   (norm_msa: eps 1e-6)
+ *     ln     = round((hidden - mean) * rstd)                         (LayerNorm without affine)
+ *     q_in   = round(round(ln * round(1 + scale[b])) + shift[b])
+ * mean and rstd (batch * seqlen, fp32) are stored when non-NULL.  gate / shift / scale are (batch, dim) views with row
+ * stride mod_rs.  dim % 4 == 0, dim <= 2048; alignment as the block tail's.  batch == 0 or seqlen == 0 passes the checks and
+ * launches nothing.  One 128-thread CTA per token row (the four-warps-per-row layout of the block tail). */
+typedef struct {
+    const void *x, *mix, *gate, *shift, *scale;
+    const int32_t *rowmap;
+    void *hidden, *q_in;
+    float *mean, *rstd;
+    int64_t mod_rs;
+    int32_t batch, seqlen, dim, dtype;
+    float eps;
+} zg_text_prologue_params;
+
+int zg_text_prologue_fwd(const zg_text_prologue_params *p, void *stream);
+
+/* Backward of the above.  Inputs d_hidden (the gradient reaching hidden from the next block's tail, NULL = zero) and d_q
+ * (the gradient of q_in); hidden, mean and rstd from the forward; mix read through rowmap as in the forward:
+ *     d_ln = round(d_q * round(1 + scale[b]))        dshift[b] += sum_l d_q        dscale[b] += sum_l d_q * ln
+ *     g    = (d_ln - (xhat * mean(d_ln * xhat) + mean(d_ln))) * rstd       xhat = (hidden - mean) * rstd   (LayerNorm bwd)
+ *     dh   = round(d_hidden + round(g));   d_x = dh
+ *     d_mix[b, rowmap[l]] = round(gate[b] * dh[b, l])                        dgate[b] += sum_l dh[b, l] * mix[b, rowmap[l]]
+ * dgate / dshift / dscale are (batch, dim) fp32 accumulated with atomics (caller zero-fills; any may be NULL).  The kernel
+ * runs nparts persistent 128-thread CTAs (1 <= nparts <= 65535) with the partition of zg_block_tail_bwd.  dim % 4 == 0,
+ * dim <= 1024.  The _det twin follows the deterministic contract above: one partial row per warp index within a batch
+ * element, the workspace holds 4 * nparts / batch rows of batch * dim floats (each rounded up to 16 bytes) for every
+ * non-NULL column sum, and it needs 4 * nparts >= batch. */
+typedef struct {
+    const void *d_hidden, *d_q;
+    const void *hidden, *mix, *gate, *scale;
+    const float *mean, *rstd;
+    const int32_t *rowmap;
+    void *d_x, *d_mix;
+    float *dgate, *dshift, *dscale;
+    int64_t mod_rs;
+    int32_t batch, seqlen, dim, dtype, nparts;
+} zg_text_prologue_bwd_params;
+
+int zg_text_prologue_bwd(const zg_text_prologue_bwd_params *p, void *stream);
+int64_t zg_text_prologue_bwd_det_workspace_bytes(const zg_text_prologue_bwd_params *p);
+int zg_text_prologue_bwd_det(const zg_text_prologue_bwd_params *p, void *workspace, int64_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

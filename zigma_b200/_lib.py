@@ -99,6 +99,20 @@ class XattnBwdParams(C.Structure):
                 + [("sms", i32)])
 
 
+class TextPrologueParams(C.Structure):
+    _fields_ = ([(n, vp) for n in ("x", "mix", "gate", "shift", "scale", "rowmap", "hidden", "q_in", "mean", "rstd")]
+                + [("mod_rs", i64)]
+                + [(n, i32) for n in ("batch", "seqlen", "dim", "dtype")]
+                + [("eps", f32)])
+
+
+class TextPrologueBwdParams(C.Structure):
+    _fields_ = ([(n, vp) for n in ("d_hidden", "d_q", "hidden", "mix", "gate", "scale", "mean", "rstd", "rowmap", "d_x", "d_mix",
+                                   "dgate", "dshift", "dscale")]
+                + [("mod_rs", i64)]
+                + [(n, i32) for n in ("batch", "seqlen", "dim", "dtype", "nparts")])
+
+
 class GemmParams(C.Structure):
     _fields_ = ([(n, vp) for n in ("A", "B", "bias", "C", "out_rowmap")]
                 + [(n, i64) for n in ("lda", "ldb", "ldc")]
@@ -115,9 +129,10 @@ class AdamWParams(C.Structure):
 EXPORTS = ["zg_abi_version", "zg_last_error", "zg_launch_count", "zg_last_scan_kernel", "zg_scan_kernel_choice", "zg_selective_scan_fwd", "zg_selective_scan_bwd",
            "zg_causal_conv1d_fwd", "zg_causal_conv1d_bwd", "zg_add_norm_fwd", "zg_add_norm_bwd",
            "zg_block_tail_fwd", "zg_block_tail_fwd_pe", "zg_block_tail_bwd", "zg_block_tail_fwd_dp", "zg_block_tail_bwd_dp",
-           "zg_gemm_bf16_tn", "zg_adamw_ema_step"]
+           "zg_gemm_bf16_tn", "zg_adamw_ema_step", "zg_text_prologue_fwd", "zg_text_prologue_bwd"]
 # deterministic backward twins (zg_<op>_det + zg_<op>_det_workspace_bytes) of these entry points
-DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd", "zg_block_tail_bwd_dp"]
+DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd", "zg_block_tail_bwd_dp",
+           "zg_text_prologue_bwd"]
 EXPORTS += [n + s for n in DET_OPS for s in ("_det", "_det_workspace_bytes")]
 # cross-attention (always atomic-free, so no _det twin); the last two have signatures of their own
 EXPORTS += ["zg_cross_attn_fwd", "zg_cross_attn_bwd", "zg_cross_attn_bwd_workspace_bytes"]

@@ -9,11 +9,18 @@ Forward: ``zg_block_tail_fwd`` (one pass, the reference's bf16 rounding points r
 ``zg_block_tail_bwd`` (one pass: RMSNorm backward, d_mix scattered back to scan order, dgate / dshift / dscale /
 d_norm_w column sums in registers).  The unfused graph costs ~12 elementwise / reduction kernels per block and
 direction (DESIGN.md section 4.4).
+
+TextPrologueFn is the text branch of a has_text block up to the cross-attention (model_zigma.py:206-208):
+
+    hidden   = x + gate * mix[:, rowmap]                          the mixer's gated residual add + un-permutation
+    q_in     = LayerNorm_noaffine(hidden) * (1 + scale) + shift    norm_msa + modulate
+
+on ``zg_text_prologue_fwd`` / ``zg_text_prologue_bwd`` (DESIGN.md section 4.7).
 """
 import torch
 
 from . import _lib
-from .engine import block_tail
+from .engine import block_tail, text_prologue
 
 
 def _contig(t):
@@ -87,3 +94,48 @@ class BlockTailFn(torch.autograd.Function):
 
 def block_tail_fn(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, path_scale=None):
     return BlockTailFn.apply(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, path_scale)
+
+
+class TextPrologueFn(torch.autograd.Function):
+    """(x, mix, gate, rowmap, shift, scale, eps) -> (hidden, q_in).  x, mix: (B, L, D) (mix in scan order, rowmap: int32 (L,)
+    or None); gate / shift / scale: (B, D) views (chunks of adaLN's output).  Every operand is brought to x.dtype, the
+    casting policy of BlockTailFn; hidden and q_in are in x.dtype.  The backward runs zg_text_prologue_bwd (its _det twin
+    under torch.use_deterministic_algorithms)."""
+
+    @staticmethod
+    def forward(ctx, x, mix, gate, rowmap, shift, scale, eps):
+        x, mix = _contig(x), _contig(mix)
+        ctx.in_dtypes = (mix.dtype, gate.dtype, shift.dtype, scale.dtype)
+        cast = lambda t: t if t.dtype == x.dtype else t.to(x.dtype)
+        mix, gate, shift, scale = cast(mix), cast(gate), cast(shift), cast(scale)
+        if any(m.stride(0) != gate.stride(0) or m.stride(1) != 1 for m in (gate, shift, scale)):
+            gate, shift, scale = gate.contiguous(), shift.contiguous(), scale.contiguous()
+        hidden, q_in, mean, rstd = text_prologue(x, mix, gate, shift, scale, rowmap, eps, want_stats=True)
+        ctx.save_for_backward(hidden, mean, rstd, mix, gate, scale, rowmap)
+        return hidden, q_in
+
+    @staticmethod
+    def backward(ctx, d_hidden, d_q):
+        hidden, mean, rstd, mix, gate, scale, rowmap = ctx.saved_tensors
+        B, L, D = hidden.shape
+        act, dev = hidden.dtype, hidden.device
+        if d_q is None:
+            d_q = torch.zeros_like(hidden)
+        d_hidden, d_q = _contig(d_hidden), _contig(d_q)
+        d_x, d_mix = torch.empty_like(hidden), torch.empty_like(hidden)
+        acc = torch.zeros((3, B, D), dtype=torch.float32, device=dev)
+        q = _lib.TextPrologueBwdParams()
+        q.d_hidden, q.d_q, q.hidden, q.mix, q.gate, q.scale = (_lib.ptr(d_hidden), _lib.ptr(d_q), _lib.ptr(hidden), _lib.ptr(mix),
+                                                               _lib.ptr(gate), _lib.ptr(scale))
+        q.mean, q.rstd, q.rowmap, q.d_x, q.d_mix = _lib.ptr(mean), _lib.ptr(rstd), _lib.ptr(rowmap), _lib.ptr(d_x), _lib.ptr(d_mix)
+        q.dgate, q.dshift, q.dscale = _lib.ptr(acc[0]), _lib.ptr(acc[1]), _lib.ptr(acc[2])
+        q.mod_rs = gate.stride(0)
+        q.batch, q.seqlen, q.dim, q.dtype = B, L, D, _lib.dt(act)
+        q.nparts = tail_bwd_nparts(B, L, torch.cuda.get_device_properties(dev).multi_processor_count)
+        _lib.call_bwd("zg_text_prologue_bwd", q)
+        dt_mix, dt_gate, dt_shift, dt_scale = ctx.in_dtypes
+        return d_x, d_mix.to(dt_mix), acc[0].to(dt_gate), None, acc[1].to(dt_shift), acc[2].to(dt_scale), None
+
+
+def text_prologue_fn(x, mix, gate, rowmap, shift, scale, eps):
+    return TextPrologueFn.apply(x, mix, gate, rowmap, shift, scale, eps)

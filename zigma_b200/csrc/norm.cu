@@ -678,6 +678,242 @@ template <typename T, bool DET> static int block_tail_bwd_t(const zg_block_tail_
     return zg_check_launch(path_scale ? "block_tail_bwd_dp" : "block_tail_bwd");
 }
 
+// ------------------------------------------------------------------------------------------------
+// Text prologue (see include/zigma_b200.h): hidden = x + gate * mix[rowmap], no-affine LayerNorm (norm_msa), modulate.
+// The four-warps-per-row layout of block_tail_row4_body: one 128-thread CTA per token row, every operand of the row loaded
+// as raw 8/16-byte vectors before the first use, the row kept in registers through the mean, the variance (two-pass, as
+// the reference's fp32 LayerNorm statistics) and the output pass.  Reads x, mix; writes hidden, q_in: 4 row passes.
+template <typename T, int MAXQ>
+__global__ void __launch_bounds__(128, (MAXQ * sizeof(T) <= 4) ? ZG_TAIL_MINB : (MAXQ * sizeof(T) <= 8) ? 8 : 5) text_prologue_fwd_kernel(const zg_text_prologue_params p) {
+    __shared__ float red[2][4];
+    const int64_t row = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int D = p.dim, nq = D >> 2;
+    const int b = (int)(row / p.seqlen), l = (int)(row % p.seqlen);
+    const T *x = reinterpret_cast<const T *>(p.x) + row * D;
+    const T *mix = reinterpret_cast<const T *>(p.mix) + ((int64_t)b * p.seqlen + (p.rowmap ? p.rowmap[l] : l)) * D;
+    const T *gate = reinterpret_cast<const T *>(p.gate) + (int64_t)b * p.mod_rs;
+    const T *shift = reinterpret_cast<const T *>(p.shift) + (int64_t)b * p.mod_rs;
+    const T *scale = reinterpret_cast<const T *>(p.scale) + (int64_t)b * p.mod_rs;
+    T *hidden = reinterpret_cast<T *>(p.hidden) + row * D;
+    T *q_in = reinterpret_cast<T *>(p.q_in) + row * D;
+    auto block_sum = [&](float v, int slot) {
+        v = zg_warp_sum(v);
+        if (lane == 0) red[slot][warp] = v;
+        __syncthreads();
+        return (red[slot][0] + red[slot][1]) + (red[slot][2] + red[slot][3]);
+    };
+    Raw4<T> rx[MAXQ], rm[MAXQ], rg[MAXQ], rsc[MAXQ], rsh[MAXQ];
+#pragma unroll
+    for (int k = 0; k < MAXQ; ++k) {
+        const int q = tid + 128 * k;
+        if (q < nq) {
+            rx[k] = ldraw<T>(x, 4 * q);
+            rm[k] = ldraw<T>(mix, 4 * q);
+            rg[k] = ldraw<T>(gate, 4 * q);
+            rsc[k] = ldraw<T>(scale, 4 * q);
+            rsh[k] = ldraw<T>(shift, 4 * q);
+        }
+    }
+    float h[MAXQ][4];
+    float sum = 0.f;
+#pragma unroll
+    for (int k = 0; k < MAXQ; ++k) {
+        const int q = tid + 128 * k;
+        if (q < nq) {
+            float m[4], g[4];
+            cvt4<T>(rx[k], h[k]);
+            cvt4<T>(rm[k], m);
+            cvt4<T>(rg[k], g);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                h[k][i] = round_to<T>(h[k][i] + round_to<T>(g[i] * m[i]));
+                sum += h[k][i];
+            }
+            st4<T>(hidden, 4 * q, h[k]);
+        }
+    }
+    const float mean = block_sum(sum, 0) / D;
+    float s2 = 0.f;
+#pragma unroll
+    for (int k = 0; k < MAXQ; ++k)
+        if (tid + 128 * k < nq)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) { const float d = h[k][i] - mean; s2 += d * d; }
+    const float rstd = 1.f / sqrtf(block_sum(s2, 1) / D + p.eps);
+    if (tid == 0) {
+        if (p.mean) p.mean[row] = mean;
+        if (p.rstd) p.rstd[row] = rstd;
+    }
+#pragma unroll
+    for (int k = 0; k < MAXQ; ++k) {
+        const int q = tid + 128 * k;
+        if (q < nq) {
+            float sc[4], sh[4], o[4];
+            cvt4<T>(rsc[k], sc);
+            cvt4<T>(rsh[k], sh);
+#pragma unroll
+            for (int i = 0; i < 4; ++i)    // modulate(ln, shift, scale) at the eager rounding points
+                o[i] = round_to<T>(round_to<T>(round_to<T>((h[k][i] - mean) * rstd) * round_to<T>(1.f + sc[i])) + sh[i]);
+            st4<T>(q_in, 4 * q, o);
+        }
+    }
+}
+
+template <typename T> static int text_prologue_fwd_t(const zg_text_prologue_params &p, cudaStream_t s) {
+    const unsigned grid = (unsigned)((int64_t)p.batch * p.seqlen);
+    if (p.dim <= 512) text_prologue_fwd_kernel<T, 1><<<grid, 128, 0, s>>>(p);
+    else if (p.dim <= 1024) text_prologue_fwd_kernel<T, 2><<<grid, 128, 0, s>>>(p);
+    else if (p.dim <= 1536) text_prologue_fwd_kernel<T, 3><<<grid, 128, 0, s>>>(p);
+    else text_prologue_fwd_kernel<T, 4><<<grid, 128, 0, s>>>(p);
+    zg_count_launch();
+    return zg_check_launch("text_prologue_fwd");
+}
+
+// Backward: the persistent-warp layout and the partition of block_tail_bwd_kernel (block_tail_bwd_body.cuh) -- one warp per
+// token row, lanes own 4-column quads, contiguous row ranges (DET: warps partitioned per batch element, partial rows indexed
+// by the warp's index within its element), the three per-batch column sums in lane-private shared-memory slots, flushed
+// when the batch element changes.  The body is not shared with the tail's: its operands differ in type (hidden in the I/O
+// dtype with a saved mean against the tail's fp32 r), in the normalisation (LayerNorm without weight against RMSNorm with
+// one) and in the rounding points, and the tail's kernels keep the code they have.
+template <typename T, int MAXQ, bool DET>
+__global__ void __launch_bounds__(128, 3) text_prologue_bwd_kernel(const zg_text_prologue_bwd_params p) {
+    extern __shared__ __align__(16) float tp_smem[];
+    float4 *acc_s = reinterpret_cast<float4 *>(tp_smem) + (threadIdx.x >> 5) * (3 * MAXQ * 32) + (threadIdx.x & 31);   // [warp][3][MAXQ][32 lanes]
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    const int64_t nrows = (int64_t)p.batch * p.seqlen;
+    const int64_t per = (nrows + nwarps - 1) / nwarps;
+    const int D = p.dim, nq = D >> 2;
+    const float invD = 1.f / D;
+#pragma unroll
+    for (int k = 0; k < MAXQ; ++k)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) acc_s[(j * MAXQ + k) * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
+    auto flush_batch = [&](int b) {
+#pragma unroll
+        for (int k = 0; k < MAXQ; ++k) {
+            const int q = lane + 32 * k;
+            if (q < nq) {
+                float *dst[3] = {p.dgate, p.dshift, p.dscale};
+#pragma unroll
+                for (int j = 0; j < 3; ++j) {
+                    const float4 v = acc_s[(j * MAXQ + k) * 32];
+                    if (DET && dst[j]) {
+                        *reinterpret_cast<float4 *>(dst[j] + ((warp % (nwarps / p.batch)) * p.batch + b) * D + 4 * q) = v;
+                    } else if (dst[j]) {
+                        float *o = dst[j] + (int64_t)b * D + 4 * q;
+                        atomicAdd(o, v.x); atomicAdd(o + 1, v.y); atomicAdd(o + 2, v.z); atomicAdd(o + 3, v.w);
+                    }
+                    acc_s[(j * MAXQ + k) * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
+                }
+            }
+        }
+    };
+    int64_t row0 = min(warp * per, nrows), row1 = min(row0 + per, nrows);
+    if constexpr (DET) {
+        const int64_t wpb = nwarps / p.batch, bw = warp / wpb, per_b = (p.seqlen + wpb - 1) / wpb;
+        row0 = row1 = nrows;
+        if (bw < p.batch) {
+            row0 = bw * p.seqlen + min((warp % wpb) * per_b, (int64_t)p.seqlen);
+            row1 = bw * p.seqlen + min((warp % wpb + 1) * per_b, (int64_t)p.seqlen);
+            if (row0 == row1) flush_batch((int)bw);      // no rows: this warp's partial rows are zeros
+        }
+    }
+    if (row0 >= row1) return;
+    int cur_b = (int)(row0 / p.seqlen);
+    for (int64_t row = row0; row < row1; ++row) {
+        const int b = (int)(row / p.seqlen), l = (int)(row % p.seqlen);
+        if (b != cur_b) { flush_batch(cur_b); cur_b = b; }
+        const int64_t mrow = (int64_t)b * p.seqlen + (p.rowmap ? p.rowmap[l] : l);
+        const T *hid = reinterpret_cast<const T *>(p.hidden) + row * D;
+        const T *dq = reinterpret_cast<const T *>(p.d_q) + row * D;
+        const T *dhid = p.d_hidden ? reinterpret_cast<const T *>(p.d_hidden) + row * D : nullptr;
+        const T *mix = reinterpret_cast<const T *>(p.mix) + mrow * D;
+        const T *gate = reinterpret_cast<const T *>(p.gate) + (int64_t)b * p.mod_rs;
+        const T *scale = reinterpret_cast<const T *>(p.scale) + (int64_t)b * p.mod_rs;
+        const float mean = p.mean[row], rstd = p.rstd[row];
+        Raw4<T> rh[MAXQ], rdq[MAXQ], rdh[MAXQ], rmx[MAXQ];
+#pragma unroll
+        for (int k = 0; k < MAXQ; ++k) {
+            const int q = lane + 32 * k;
+            if (q < nq) {
+                rh[k] = ldraw<T>(hid, 4 * q);
+                rdq[k] = ldraw<T>(dq, 4 * q);
+                if (dhid) rdh[k] = ldraw<T>(dhid, 4 * q);
+                rmx[k] = ldraw<T>(mix, 4 * q);
+            }
+        }
+        // ---- d_ln, dshift / dscale, the two LayerNorm-backward row means ----
+        float dl[MAXQ][4];
+        float c1 = 0.f, c2 = 0.f;
+#pragma unroll
+        for (int k = 0; k < MAXQ; ++k) {
+            const int q = lane + 32 * k;
+            if (q < nq) {
+                float hv[4], g[4], sc[4];
+                cvt4<T>(rh[k], hv);
+                cvt4<T>(rdq[k], g);
+                ld4<T>(scale, 4 * q, sc);
+                float4 ash = acc_s[(1 * MAXQ + k) * 32], asc = acc_s[(2 * MAXQ + k) * 32];
+                float *psh = &ash.x, *psc = &asc.x;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float xh = (hv[i] - mean) * rstd;
+                    dl[k][i] = round_to<T>(g[i] * round_to<T>(1.f + sc[i]));
+                    psh[i] += g[i];
+                    psc[i] = fmaf(g[i], round_to<T>(xh), psc[i]);      // d_q * ln
+                    c1 = fmaf(xh, dl[k][i], c1);
+                    c2 += dl[k][i];
+                }
+                acc_s[(1 * MAXQ + k) * 32] = ash; acc_s[(2 * MAXQ + k) * 32] = asc;
+            }
+        }
+        c1 = zg_warp_sum(c1) * invD;
+        c2 = zg_warp_sum(c2) * invD;
+        // ---- dh, d_x, d_mix, dgate ----
+        T *dx = reinterpret_cast<T *>(p.d_x) + row * D;
+        T *dmix = reinterpret_cast<T *>(p.d_mix) + mrow * D;
+#pragma unroll
+        for (int k = 0; k < MAXQ; ++k) {
+            const int q = lane + 32 * k;
+            if (q < nq) {
+                float hv[4], dh[4], m[4], g[4], o[4];
+                cvt4<T>(rh[k], hv);
+                if (dhid) cvt4<T>(rdh[k], dh);
+                else dh[0] = dh[1] = dh[2] = dh[3] = 0.f;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float xh = (hv[i] - mean) * rstd;
+                    dh[i] = round_to<T>(dh[i] + round_to<T>((dl[k][i] - (xh * c1 + c2)) * rstd));
+                }
+                st4<T>(dx, 4 * q, dh);
+                cvt4<T>(rmx[k], m);
+                ld4<T>(gate, 4 * q, g);
+                float4 ag = acc_s[(0 * MAXQ + k) * 32];
+                float *pg = &ag.x;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) { o[i] = g[i] * dh[i]; pg[i] = fmaf(dh[i], m[i], pg[i]); }
+                acc_s[(0 * MAXQ + k) * 32] = ag;
+                st4<T>(dmix, 4 * q, o);
+            }
+        }
+    }
+    flush_batch(cur_b);
+}
+
+template <typename T, bool DET> static int text_prologue_bwd_t(const zg_text_prologue_bwd_params &p, cudaStream_t s) {
+    const unsigned grid = (unsigned)p.nparts;
+    // dynamic shared memory: 4 warps x 3 accumulator sets x MAXQ quads x 32 lanes x 16 B  (48 KB at MAXQ 8)
+    if (p.dim <= 512) text_prologue_bwd_kernel<T, 4, DET><<<grid, 128, 4 * 3 * 4 * 32 * 16, s>>>(p);
+    else if (p.dim <= 640) text_prologue_bwd_kernel<T, 5, DET><<<grid, 128, 4 * 3 * 5 * 32 * 16, s>>>(p);
+    else if (p.dim <= 768) text_prologue_bwd_kernel<T, 6, DET><<<grid, 128, 4 * 3 * 6 * 32 * 16, s>>>(p);
+    else text_prologue_bwd_kernel<T, 8, DET><<<grid, 128, 4 * 3 * 8 * 32 * 16, s>>>(p);
+    zg_count_launch();
+    return zg_check_launch("text_prologue_bwd");
+}
+
 template <typename T, typename R> static int norm_fwd_tr(const zg_norm_params &p, cudaStream_t s) {
     const int64_t nthreads = (int64_t)p.nrows * 32;
     add_norm_fwd_kernel<T, R><<<(unsigned)((nthreads + 127) / 128), 128, 0, s>>>(p);
@@ -954,4 +1190,93 @@ extern "C" int64_t zg_block_tail_bwd_dp_det_workspace_bytes(const zg_block_tail_
 extern "C" int zg_block_tail_bwd_dp_det(const zg_block_tail_bwd_dp_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
     if (int rc = block_tail_bwd_dp_validate(pp)) return rc;
     return block_tail_bwd_det_run(pp->base, pp->path_scale, workspace, workspace_bytes, stream);
+}
+
+static int text_prologue_fwd_validate(const zg_text_prologue_params &p) {
+    ZG_REQUIRE(p.x && p.mix && p.gate && p.shift && p.scale && p.hidden && p.q_in, "text_prologue_fwd: null tensor pointer");
+    ZG_REQUIRE(p.batch >= 0 && p.seqlen >= 0, "text_prologue_fwd: negative batch or seqlen");
+    ZG_REQUIRE(p.dim > 0 && p.dim % 4 == 0 && p.dim <= 4 * 32 * zg::NORM_MAXQ, "text_prologue_fwd: dim must be a multiple of 4 and <= %d, got %d",
+               4 * 32 * zg::NORM_MAXQ, p.dim);
+    ZG_REQUIRE(p.mod_rs % 4 == 0, "text_prologue_fwd: modulation row stride must be a multiple of 4");
+    ZG_REQUIRE(p.dtype == ZG_F32 || p.dtype == ZG_F16 || p.dtype == ZG_BF16, "text_prologue_fwd: bad dtype %d", p.dtype);
+    ZG_REQUIRE(aligned16(p.x) && aligned16(p.mix) && aligned16(p.hidden) && aligned16(p.q_in), "text_prologue_fwd: row tensors must be 16-byte aligned");
+    ZG_REQUIRE(aligned_quad(p.gate, p.dtype) && aligned_quad(p.shift, p.dtype) && aligned_quad(p.scale, p.dtype),
+               "text_prologue_fwd: gate / shift / scale must be aligned to 4 elements");
+    ZG_REQUIRE((int64_t)p.batch * p.seqlen <= 0x7fffffffLL, "text_prologue_fwd: fewer than 2^31 rows only");
+    return 0;
+}
+
+extern "C" int zg_text_prologue_fwd(const zg_text_prologue_params *pp, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "text_prologue_fwd: null params");
+    const zg_text_prologue_params &p = *pp;
+    if (int rc = text_prologue_fwd_validate(p)) return rc;
+    if (p.batch == 0 || p.seqlen == 0) return 0;
+    cudaStream_t s = (cudaStream_t)stream;
+    switch (p.dtype) {
+        case ZG_F32: return zg::text_prologue_fwd_t<float>(p, s);
+        case ZG_F16: return zg::text_prologue_fwd_t<__half>(p, s);
+        default: return zg::text_prologue_fwd_t<__nv_bfloat16>(p, s);
+    }
+}
+
+static int text_prologue_bwd_validate(const zg_text_prologue_bwd_params &p) {
+    ZG_REQUIRE(p.d_q && p.hidden && p.mix && p.gate && p.scale && p.mean && p.rstd && p.d_x && p.d_mix, "text_prologue_bwd: null tensor pointer");
+    ZG_REQUIRE(p.batch >= 0 && p.seqlen >= 0, "text_prologue_bwd: negative batch or seqlen");
+    ZG_REQUIRE(p.dim > 0 && p.dim % 4 == 0 && p.dim <= 1024, "text_prologue_bwd: dim must be a multiple of 4 and <= 1024, got %d", p.dim);
+    ZG_REQUIRE(p.mod_rs % 4 == 0, "text_prologue_bwd: modulation row stride must be a multiple of 4");
+    ZG_REQUIRE(p.nparts >= 1 && p.nparts <= 65535, "text_prologue_bwd: nparts (CTAs) must be in [1, 65535]");
+    ZG_REQUIRE(p.dtype == ZG_F32 || p.dtype == ZG_F16 || p.dtype == ZG_BF16, "text_prologue_bwd: bad dtype %d", p.dtype);
+    ZG_REQUIRE(aligned16(p.d_hidden) && aligned16(p.d_q) && aligned16(p.hidden) && aligned16(p.mix) && aligned16(p.d_x) && aligned16(p.d_mix),
+               "text_prologue_bwd: row tensors must be 16-byte aligned");
+    ZG_REQUIRE(aligned_quad(p.gate, p.dtype) && aligned_quad(p.scale, p.dtype), "text_prologue_bwd: gate / scale must be aligned to 4 elements");
+    return 0;
+}
+
+template <bool DET> static int text_prologue_bwd_dispatch(const zg_text_prologue_bwd_params &p, cudaStream_t s) {
+    switch (p.dtype) {
+        case ZG_F32: return zg::text_prologue_bwd_t<float, DET>(p, s);
+        case ZG_F16: return zg::text_prologue_bwd_t<__half, DET>(p, s);
+        default: return zg::text_prologue_bwd_t<__nv_bfloat16, DET>(p, s);
+    }
+}
+
+extern "C" int zg_text_prologue_bwd(const zg_text_prologue_bwd_params *pp, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "text_prologue_bwd: null params");
+    if (int rc = text_prologue_bwd_validate(*pp)) return rc;
+    if (pp->batch == 0 || pp->seqlen == 0) return 0;
+    return text_prologue_bwd_dispatch<false>(*pp, (cudaStream_t)stream);
+}
+
+// partial rows of the deterministic backward: one per warp index within a batch element (the block tail's layout)
+static ZgDetLayout text_prologue_bwd_det_layout(const zg_text_prologue_bwd_params &p, void *ws) {
+    ZgDetLayout lay;
+    lay.ws = static_cast<unsigned char *>(ws);
+    if (p.batch <= 0 || p.seqlen <= 0 || p.dim <= 0 || p.nparts < 1) return lay;
+    const int64_t wpb = 4 * (int64_t)p.nparts / p.batch, n = (int64_t)p.batch * p.dim;
+    lay.add(p.dgate, wpb, n);
+    lay.add(p.dshift, wpb, n);
+    lay.add(p.dscale, wpb, n);
+    return lay;
+}
+
+extern "C" int64_t zg_text_prologue_bwd_det_workspace_bytes(const zg_text_prologue_bwd_params *p) {
+    return p ? text_prologue_bwd_det_layout(*p, nullptr).bytes : 0;
+}
+
+extern "C" int zg_text_prologue_bwd_det(const zg_text_prologue_bwd_params *pp, void *workspace, int64_t workspace_bytes, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "text_prologue_bwd_det: null params");
+    if (int rc = text_prologue_bwd_validate(*pp)) return rc;
+    if (pp->batch == 0 || pp->seqlen == 0) return 0;
+    ZG_REQUIRE(4 * (int64_t)pp->nparts >= pp->batch, "text_prologue_bwd_det: needs at least one warp per batch element (4 * nparts >= batch), got nparts %d for batch %d",
+               pp->nparts, pp->batch);
+    const ZgDetLayout lay = text_prologue_bwd_det_layout(*pp, workspace);
+    ZG_REQUIRE_WORKSPACE(lay, workspace, workspace_bytes, "text_prologue_bwd_det");
+    zg_text_prologue_bwd_params p = *pp;        // the kernel writes partial rows; the reduction adds them to the outputs
+    int i = 0;
+    if (p.dgate) p.dgate = lay.reg[i++].part;
+    if (p.dshift) p.dshift = lay.reg[i++].part;
+    if (p.dscale) p.dscale = lay.reg[i++].part;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = text_prologue_bwd_dispatch<true>(p, s)) return rc;
+    return lay.reduce(s);
 }

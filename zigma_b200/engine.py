@@ -120,6 +120,35 @@ def block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, final=
     return res_out, normed, modded
 
 
+def text_prologue(x, mix, gate, shift, scale, rowmap, eps, mod_div=1, want_stats=False):
+    """zg_text_prologue_fwd wrapper, the text branch of a has_text block up to the attention (model_zigma.py:206-208):
+    hidden = x + gate * mix[:, rowmap];  q_in = modulate(LayerNorm_noaffine(hidden, eps), shift, scale).
+    x, mix: (Bt, L, D) contiguous in one dtype; rowmap: int32 (L,) or None; gate / shift / scale: (Bt // mod_div, D) views in
+    that dtype with a common row stride.  Returns hidden, q_in (and the fp32 (Bt * L,) mean, rstd when want_stats)."""
+    _lib.require_cuda(x, mix, gate, shift, scale, rowmap)
+    Bt, L, D = x.shape
+    if mod_div != 1:
+        # modulation vectors are per ORIGINAL batch element; expand to the folded batch (tiny), as block_tail does
+        gate, shift, scale = (m.repeat_interleave(mod_div, dim=0) for m in (gate, shift, scale))
+    if any(t.dtype != x.dtype for t in (mix, gate, shift, scale)) or tuple(mix.shape) != (Bt, L, D) or not mix.is_contiguous():
+        raise RuntimeError("text_prologue: mix must be a contiguous tensor of x's shape and every operand in x's dtype")
+    rs = gate.stride(0)
+    if any(m.stride(0) != rs or m.stride(1) != 1 or tuple(m.shape) != (Bt, D) for m in (gate, shift, scale)):
+        raise RuntimeError("text_prologue: gate / shift / scale must be (batch, dim) views sharing one row stride")
+    hidden, q_in = torch.empty_like(x), torch.empty_like(x)
+    mean = torch.empty((Bt * L,), dtype=torch.float32, device=x.device) if want_stats else None
+    rstd = torch.empty((Bt * L,), dtype=torch.float32, device=x.device) if want_stats else None
+    p = _lib.TextPrologueParams()
+    p.x, p.mix, p.gate, p.shift, p.scale, p.rowmap = _lib.ptr(x), _lib.ptr(mix), _lib.ptr(gate), _lib.ptr(shift), _lib.ptr(scale), _lib.ptr(rowmap)
+    p.hidden, p.q_in, p.mean, p.rstd = _lib.ptr(hidden), _lib.ptr(q_in), _lib.ptr(mean), _lib.ptr(rstd)
+    p.mod_rs = rs
+    p.batch, p.seqlen, p.dim, p.dtype, p.eps = Bt, L, D, _lib.dt(x), float(eps)
+    _lib.call("zg_text_prologue_fwd", p)
+    if want_stats:
+        return hidden, q_in, mean, rstd
+    return hidden, q_in
+
+
 class ZigMaEngine:
     def __init__(self, model):
         self.m = model
@@ -350,13 +379,14 @@ class ZigMaEngine:
                 # reads it; the attention branch (zg_cross_attn_fwd on the text tokens) then takes the place of the mixer output
                 # in the fused tail:  hidden2 = hidden + gate_msa * msa(modulate(norm_msa(hidden)))
                 blk = m.blocks[i]
-                # un-permute the mixer output with the layer's own row table: (B fold, L / fold) rows for a spatial video layer
-                # (same memory as (B, L)), the composite (k T + t) table of a copy-free temporal layer, the zigzag table otherwise
-                mixed = mix if rowmap is None else mix.reshape(-1, rowmap.numel(), D).index_select(1, rowmap.long())
-                hidden = normed + gate.unsqueeze(1) * mixed.reshape(B, L, D)
+                # one kernel un-permutes the mixer output with the layer's own row table -- (B fold, L / fold) rows for a spatial
+                # video layer (same memory as (B, L)), the composite (k T + t) table of a copy-free temporal layer, the zigzag
+                # table otherwise -- and forms hidden and the attention's query input
+                Bf = B * fold
+                hidden, q_in = text_prologue(normed.view(Bf, L // fold, D), mix.view(Bf, L // fold, D), gate, mods[:, i, 3], mods[:, i, 4],
+                                             rowmap, blk.norm_msa.eps, mod_div=fold)
                 fold = 1
-                q_in = blk.norm_msa(hidden) * (1 + mods[:, i, 4].unsqueeze(1)) + mods[:, i, 3].unsqueeze(1)
-                mix, rowmap, gate, normed = blk.msa(q_in, text=text, mask=None).contiguous(), None, mods[:, i, 5], hidden
+                mix, rowmap, gate, normed = blk.msa(q_in.view(B, L, D), text=text, mask=None).contiguous(), None, mods[:, i, 5], hidden.view(B, L, D)
             if fold != 1:     # spatial video layer: rows are (b t, k); same memory as (b, t k)
                 Bf = B * fold
                 residual, normed, modded = block_tail(normed.view(Bf, L // fold, D), mix, gate, shift, scale, nw,

@@ -435,35 +435,39 @@ class ZigMa(nn.Module):
                 and isinstance(self.norm_f, RMSNorm))
 
     def _fused_tail_ok(self, hidden_states):
-        """The fused training loop (block_ops.BlockTailFn) covers the configuration every shipped config uses, in eval and in
-        train mode (stochastic depth included)."""
+        """The fused training loop (block_ops.BlockTailFn, and TextPrologueFn for the text branch of has_text blocks) covers
+        the configuration every shipped config uses, in eval and in train mode (stochastic depth included)."""
         import os
         D = hidden_states.shape[-1]
-        return (hidden_states.is_cuda and self.fused_add_norm and self.residual_in_fp32 and not self.has_text and self.use_pe != 3
+        return (hidden_states.is_cuda and self.fused_add_norm and self.residual_in_fp32 and self.use_pe != 3
                 and not self.use_checkpoint and D % 4 == 0 and D <= 1024 and hidden_states.dtype in (torch.float32, torch.bfloat16, torch.float16)
                 and all(isinstance(b.norm, RMSNorm) and b.skip_linear is None for b in self.blocks)
                 and isinstance(self.norm_f, RMSNorm) and os.environ.get("ZIGMA_FUSED_TRAIN_TAIL", "1") != "0")
 
-    def _forward_fused_tail(self, hidden_states, c):
+    def _forward_fused_tail(self, hidden_states, c, text=None):
         """Same function as the block loop of forward_autograd: each block's add+norm+modulate and the PREVIOUS block's
         gated residual add + un-permutation run as one kernel (forward and backward).  A block with an active DropPath
         (training, drop_prob > 0, a residual to join) draws its multipliers here, at the point Block.forward would, and
-        its tail applies them (block_tail_fn's path_scale)."""
-        from .block_ops import block_tail_fn
+        its tail applies them (block_tail_fn's path_scale).  In a has_text block the mixer's gated residual add,
+        un-permutation, norm_msa and modulate run as one kernel (text_prologue_fn) before the cross-attention, whose
+        output then enters the next tail as its mix (gate: the attention gate, no row table)."""
+        from .block_ops import block_tail_fn, text_prologue_fn
         from .mamba_simple import permute_along
         residual, mix, gate, rowmap = None, None, None, None
         x = hidden_states.contiguous()
         for block in self.blocks:
-            mods = block.adaLN_modulation(c)
-            shift, scale, gate_next = mods.chunk(3, dim=1)
+            mods = block.adaLN_modulation(c).chunk(6 if block.has_text else 3, dim=1)
             dp = block.drop_path
             path_scale = None
             if residual is not None and isinstance(dp, DropPath) and dp.training and dp.drop_prob > 0.0:
                 path_scale = dp.draw(x).reshape(x.shape[0])     # x: the dtype the kernel forms hidden in
-            residual, x, modded = block_tail_fn(x, mix, gate, shift, scale, block.norm.weight, residual, rowmap, block.norm.eps,
+            residual, x, modded = block_tail_fn(x, mix, gate, mods[0], mods[1], block.norm.weight, residual, rowmap, block.norm.eps,
                                                 path_scale)
             mix, rowmap = block.mixer.forward_scan_order(modded)
-            gate = gate_next
+            gate = mods[2]
+            if block.has_text:
+                x, q_in = text_prologue_fn(x, mix, gate, rowmap, mods[3], mods[4], block.norm_msa.eps)
+                mix, gate, rowmap = block.msa(q_in, text=text, mask=None), mods[5], None
         if rowmap is not None:
             mix = permute_along(mix, rowmap.long(), 1)
         return x + gate.unsqueeze(1) * mix, residual
@@ -472,7 +476,7 @@ class ZigMa(nn.Module):
         hidden_states, c, y = self.embed(hidden_states, t, y)
         residual = None
         if self._fused_tail_ok(hidden_states):
-            hidden_states, residual = self._forward_fused_tail(hidden_states, c)
+            hidden_states, residual = self._forward_fused_tail(hidden_states, c, y)
             return self._forward_head(hidden_states, residual, c)
         for layer_idx, block in enumerate(self.blocks):
             if self.use_pe == 3:
