@@ -76,11 +76,16 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
-// arrive on the barrier at this shared-memory offset in CTA `cta` of the cluster
+// arrive on the barrier at this shared-memory offset in CTA `cta` of the cluster.  Only ever used to hand a ring stage back to
+// the producers, and for that the default (.release.cta) ordering is enough: the shared-memory reads being released are wgmma
+// (async-proxy) reads that wgmma.wait_group has already retired before the arrive, this thread made no generic writes to the
+// stage, and the producer that overwrites it acquires the barrier phase (try_wait) before it issues the TMA.  A .release.cluster
+// arrive would compile to a GPU-wide memory barrier (MEMBAR.ALL.GPU) per arrive, i.e. per consumer warp and k-block, which
+// also has to wait for the epilogue's outstanding global stores.
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t *bar, uint32_t cta) {
     uint32_t ra;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(cta));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
