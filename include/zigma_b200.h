@@ -324,6 +324,21 @@ typedef struct {
 } zg_block_tail_bwd_dp_params;
 
 int zg_block_tail_fwd_dp(const zg_block_tail_dp_params *p, void *stream);
+
+/* Block tail whose x is the previous tail's normed output, rebuilt instead of read: with r_prev = this call's residual (the previous
+ * tail's residual_out), rstd_prev and w_prev the previous tail's rstd and norm_w,
+ *     x = round_to_dtype(r_prev * rstd_prev[row] * w_prev)      -- the previous tail's normed, bit for bit
+ * then everything as zg_block_tail_fwd.  So a chain of tails needs no normed tensor between them: each passes its rstd on, and
+ * writes normed only where something else reads it.  Saves a (batch, seqlen, dim) write and read per tail.
+ *   base.x: NULL.  base.residual: required.  base.normed: may be NULL unless final_layer.  dim <= 1024.
+ *   x_rstd: (batch * seqlen) fp32, 4-byte aligned.  x_norm_w: (dim) in dtype, aligned to 4 elements. */
+typedef struct {
+    zg_block_tail_params base;
+    const float *x_rstd;
+    const void *x_norm_w;
+} zg_block_tail_rebuild_params;
+
+int zg_block_tail_fwd_rebuild(const zg_block_tail_rebuild_params *p, void *stream);
 int zg_block_tail_bwd_dp(const zg_block_tail_bwd_dp_params *p, void *stream);
 int64_t zg_block_tail_bwd_dp_det_workspace_bytes(const zg_block_tail_bwd_dp_params *p);
 int zg_block_tail_bwd_dp_det(const zg_block_tail_bwd_dp_params *p, void *workspace, int64_t workspace_bytes, void *stream);

@@ -86,6 +86,10 @@ class BlockTailBwdDpParams(C.Structure):
     _fields_ = [("base", BlockTailBwdParams), ("path_scale", vp)]
 
 
+class BlockTailRebuildParams(C.Structure):
+    _fields_ = [("base", BlockTailParams), ("x_rstd", vp), ("x_norm_w", vp)]
+
+
 class XattnParams(C.Structure):
     _fields_ = ([(n, vp) for n in ("q", "k", "v", "o", "lse")]
                 + [(n, i64) for n in ("q_sb", "q_rs", "k_sb", "k_rs", "v_sb", "v_rs", "o_sb", "o_rs")]
@@ -129,6 +133,7 @@ class AdamWParams(C.Structure):
 EXPORTS = ["zg_abi_version", "zg_last_error", "zg_launch_count", "zg_last_scan_kernel", "zg_scan_kernel_choice", "zg_selective_scan_fwd", "zg_selective_scan_bwd",
            "zg_causal_conv1d_fwd", "zg_causal_conv1d_bwd", "zg_add_norm_fwd", "zg_add_norm_bwd",
            "zg_block_tail_fwd", "zg_block_tail_fwd_pe", "zg_block_tail_bwd", "zg_block_tail_fwd_dp", "zg_block_tail_bwd_dp",
+           "zg_block_tail_fwd_rebuild",
            "zg_gemm_bf16_tn", "zg_adamw_ema_step", "zg_text_prologue_fwd", "zg_text_prologue_bwd"]
 # deterministic backward twins (zg_<op>_det + zg_<op>_det_workspace_bytes) of these entry points
 DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "zg_block_tail_bwd", "zg_block_tail_bwd_dp",

@@ -446,14 +446,17 @@ __global__ void __launch_bounds__(128, (MAXQ <= 6) ? 6 : 1) block_tail_kernel(co
 // (model_zigma.py:941), without an elementwise pass of its own.  A separate instantiation: the per-layer instance is unchanged.
 // DP (zg_block_tail_fwd_dp, stochastic depth in training): hidden is multiplied by the batch element's drop-path multiplier
 // before the residual add, kept = round(hidden * path_scale[b]), the reference's eager `x * mask`.  One scalar load per row.
-template <typename T, int MAXQ, bool PE, bool DP>
-__device__ __forceinline__ void block_tail_row4_body(const zg_block_tail_params &p, const void *path_scale) {
+// RB (zg_block_tail_fwd_rebuild): x is not read; it is the previous tail's normed output, rebuilt from the residual row this
+// kernel loads anyway as round(residual * x_rstd[row] * x_norm_w), the previous tail's own expression on the same operands.
+template <typename T, int MAXQ, bool PE, bool DP, bool RB = false>
+__device__ __forceinline__ void block_tail_row4_body(const zg_block_tail_params &p, const void *path_scale, const float *x_rstd = nullptr,
+                                                     const void *x_norm_w = nullptr) {
     __shared__ float red[3][4];
     const int64_t row = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int D = p.dim, nq = D >> 2;
     const int b = (int)(row / p.seqlen), l = (int)(row % p.seqlen);
-    const T *x = reinterpret_cast<const T *>(p.x) + row * D;
+    const T *x = RB ? reinterpret_cast<const T *>(x_norm_w) : reinterpret_cast<const T *>(p.x) + row * D;   // RB: per column
     const T *mix = nullptr;
     if (p.mix) {
         const int64_t src = (PE ? 0 : (int64_t)b * p.seqlen) + (p.rowmap ? p.rowmap[l] : l);
@@ -486,22 +489,32 @@ __device__ __forceinline__ void block_tail_row4_body(const zg_block_tail_params 
         if (q < nq) {
             rx[k] = ldraw<T>(x, 4 * q);
             if (mix) { rm[k] = ldraw<T>(mix, 4 * q); rg[k] = PE ? raw_ones<T>() : ldraw<T>(gate, 4 * q); }     // PE: gate = 1, round(1 * m) = m
-            if (res) rr[k] = *reinterpret_cast<const float4 *>(res + 4 * q);
+            if (RB || res) rr[k] = *reinterpret_cast<const float4 *>(res + 4 * q);
             rw[k] = ldraw<T>(nw, 4 * q);
 #if ZG_TAIL_PREFETCH_MOD
-            if (modded) { rsc[k] = ldraw<T>(scale, 4 * q); rsh[k] = ldraw<T>(shift, 4 * q); }
+            if (!RB && modded) { rsc[k] = ldraw<T>(scale, 4 * q); rsh[k] = ldraw<T>(shift, 4 * q); }   // (RB: 40 registers without spills)
 #endif
         }
     }
     float dps = 1.f;
     if constexpr (DP) dps = zg_to_float<T>(reinterpret_cast<const T *>(path_scale)[b]);
+    float xrs = 0.f;
+    if constexpr (RB) xrs = x_rstd[row];
     float r[MAXQ][4];
     float sumsq = 0.f;
 #pragma unroll
     for (int k = 0; k < MAXQ; ++k) {
         const int q = tid + 128 * k;
         if (q < nq) {
-            cvt4<T>(rx[k], r[k]);
+            if constexpr (RB) {
+                float w[4];
+                const float rp[4] = {rr[k].x, rr[k].y, rr[k].z, rr[k].w};
+                cvt4<T>(rx[k], w);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) r[k][i] = round_to<T>(__fmul_rn(__fmul_rn(rp[i], xrs), w[i]));   // no FMA: the stored product
+            } else {
+                cvt4<T>(rx[k], r[k]);
+            }
             if (mix) {
                 float m[4], g[4];
                 cvt4<T>(rm[k], m);
@@ -514,7 +527,7 @@ __device__ __forceinline__ void block_tail_row4_body(const zg_block_tail_params 
 #pragma unroll
                 for (int i = 0; i < 4; ++i) r[k][i] = round_to<T>(__fmul_rn(r[k][i], dps));   // rounded before the add (no FMA)
             }
-            if (res) {
+            if (RB || res) {
                 r[k][0] += rr[k].x; r[k][1] += rr[k].y; r[k][2] += rr[k].z; r[k][3] += rr[k].w;
             }
             if (rout) st4<float>(rout, 4 * q, r[k]);
@@ -564,12 +577,17 @@ __device__ __forceinline__ void block_tail_row4_body(const zg_block_tail_params 
     for (int k = 0; k < MAXQ; ++k) {
         const int q = tid + 128 * k;
         if (q < nq) {
-            st4<T>(normed, 4 * q, r[k]);
+            if (!RB || p.normed) st4<T>(normed, 4 * q, r[k]);      // (RB: normed may be NULL below the final layer)
             if (modded) {
                 float sc[4], sh[4], o[4];
 #if ZG_TAIL_PREFETCH_MOD
-                cvt4<T>(rsc[k], sc);
-                cvt4<T>(rsh[k], sh);
+                if constexpr (RB) {
+                    ld4<T>(scale, 4 * q, sc);
+                    ld4<T>(shift, 4 * q, sh);
+                } else {
+                    cvt4<T>(rsc[k], sc);
+                    cvt4<T>(rsh[k], sh);
+                }
 #else
                 ld4<T>(scale, 4 * q, sc);
                 ld4<T>(shift, 4 * q, sh);
@@ -591,6 +609,20 @@ __global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_row4_kernel(cons
 template <typename T, int MAXQ>
 __global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_dp_fwd_kernel(const zg_block_tail_dp_params p) {
     block_tail_row4_body<T, MAXQ, false, true>(p.base, p.path_scale);
+}
+
+template <typename T, int MAXQ>
+__global__ void __launch_bounds__(128, ZG_TAIL_MINB) block_tail_rebuild_fwd_kernel(const zg_block_tail_rebuild_params p) {
+    block_tail_row4_body<T, MAXQ, false, false, true>(p.base, nullptr, p.x_rstd, p.x_norm_w);
+}
+
+// zg_block_tail_fwd_rebuild: the four-warps-per-row kernel only (dim <= 1024 -> Q 1 or 2, checked by the entry point)
+template <typename T> static int block_tail_rebuild_t(const zg_block_tail_rebuild_params &p, cudaStream_t s) {
+    const unsigned g4 = (unsigned)((int64_t)p.base.batch * p.base.seqlen);
+    if (p.base.dim <= 512) block_tail_rebuild_fwd_kernel<T, 1><<<g4, 128, 0, s>>>(p);
+    else block_tail_rebuild_fwd_kernel<T, 2><<<g4, 128, 0, s>>>(p);
+    zg_count_launch();
+    return zg_check_launch("block_tail_fwd_rebuild");
 }
 
 // zg_block_tail_fwd_dp: the four-warps-per-row kernel only (dim <= 1024 -> Q 1 or 2, checked by the entry point)
@@ -1037,8 +1069,8 @@ extern "C" int zg_add_norm_bwd_det(const zg_norm_bwd_params *pp, void *workspace
     return lay.reduce(s);
 }
 
-static int block_tail_fwd_validate(const zg_block_tail_params &p, bool pe) {
-    ZG_REQUIRE(p.x && p.norm_w && p.normed, "block_tail_fwd: null tensor pointer");
+static int block_tail_fwd_validate(const zg_block_tail_params &p, bool pe, bool rebuild = false) {
+    ZG_REQUIRE((rebuild || (p.x && p.normed)) && p.norm_w, "block_tail_fwd: null tensor pointer");
     if (pe) ZG_REQUIRE(p.mix && !p.gate && !p.rowmap && !p.residual, "block_tail_fwd_pe: takes the (seqlen, dim) table as mix and no gate / rowmap / residual");
     else ZG_REQUIRE(!p.mix || p.gate, "block_tail_fwd: mix needs gate");
     ZG_REQUIRE(!p.modded || (p.shift && p.scale), "block_tail_fwd: modded needs shift and scale");
@@ -1073,6 +1105,28 @@ extern "C" int zg_block_tail_fwd_pe(const zg_block_tail_params *pp, void *stream
 // path_scale is read as one dtype element per batch element
 static bool aligned_elem(const void *p, int dtype) {
     return (reinterpret_cast<uintptr_t>(p) & ((dtype == ZG_F32 ? sizeof(float) : sizeof(__half)) - 1)) == 0;
+}
+
+extern "C" int zg_block_tail_fwd_rebuild(const zg_block_tail_rebuild_params *pp, void *stream) {
+    ZG_REQUIRE(pp != nullptr, "block_tail_fwd_rebuild: null params");
+    const zg_block_tail_params &p = pp->base;
+    ZG_REQUIRE(p.x == nullptr, "block_tail_fwd_rebuild: x must be NULL (it is rebuilt from residual, x_rstd and x_norm_w)");
+    ZG_REQUIRE(p.residual && pp->x_rstd && pp->x_norm_w, "block_tail_fwd_rebuild: needs residual, x_rstd and x_norm_w");
+    ZG_REQUIRE(p.normed || !p.final_layer, "block_tail_fwd_rebuild: final_layer needs normed");
+    ZG_REQUIRE(p.dim <= 1024, "block_tail_fwd_rebuild: dim must be <= 1024, got %d", p.dim);
+    if (int rc = block_tail_fwd_validate(p, false, true)) return rc;
+    ZG_REQUIRE(aligned_quad(pp->x_norm_w, p.dtype) && (reinterpret_cast<uintptr_t>(pp->x_rstd) & 3) == 0,
+               "block_tail_fwd_rebuild: x_norm_w must be aligned to 4 elements, x_rstd to 4 bytes");
+    const int64_t nrows = (int64_t)p.batch * p.seqlen;
+    if (nrows == 0) return 0;
+    ZG_REQUIRE(nrows <= 0x7fffffffLL, "block_tail_fwd_rebuild: fewer than 2^31 rows only");
+    cudaStream_t s = (cudaStream_t)stream;
+    switch (p.dtype) {
+        case ZG_F32: return zg::block_tail_rebuild_t<float>(*pp, s);
+        case ZG_F16: return zg::block_tail_rebuild_t<__half>(*pp, s);
+        case ZG_BF16: return zg::block_tail_rebuild_t<__nv_bfloat16>(*pp, s);
+    }
+    return zg_set_error("block_tail_fwd_rebuild: bad dtype %d", p.dtype);
 }
 
 extern "C" int zg_block_tail_fwd_dp(const zg_block_tail_dp_params *pp, void *stream) {

@@ -8,7 +8,7 @@
 // behind it (stall `mio_throttle` 2.9-3.1 warps per issue while the MUFU pipe idles a quarter of the time).  With two channels
 // per lane the same B / C registers feed twice the recurrences: 11 wavefronts per 32 channel-steps instead of 20.6, 3 shared
 // loads + 1 store per lane-step instead of 2 x (5 + 1), half the B|C staging / conversion per channel, and ~12 % fewer issued
-// instructions per (b, e, l).  Price: ~100 registers, half the warps (4.3 per sub-partition at config 2), each with twice the
+// instructions per (b, e, l).  Price: 96 registers, half the warps (4.85 per sub-partition at config 2), each with twice the
 // independent work (16 MUFU back to back per step).
 //
 // Everything else is scan_fwd_wp.cuh: a warp stages its own u / delta / z / B|C rows (8 steps per stage, 3-deep ring, one
@@ -21,7 +21,7 @@
 namespace zg {
 
 constexpr int WP2_CH = 32;            // channels per warp
-constexpr int WP2_MAX_WARPS = 9;      // 288 threads x 2 CTAs per SM: 112 registers per thread
+constexpr int WP2_MAX_WARPS = 20;     // 640 threads, one CTA per SM: a 96-register cap, which is what ptxas allocates (no spills)
 
 struct Wp2Layout {                    // per warp
     static constexpr int NSTAGE = 3;
@@ -252,7 +252,7 @@ __device__ __forceinline__ void wp2_body(const zg_scan_params &p, unsigned char 
 }
 
 template <typename T, bool PLAIN>
-__global__ void __launch_bounds__(32 * WP2_MAX_WARPS, 2) scan_fwd_wp2_kernel(const zg_scan_params p) {
+__global__ void __launch_bounds__(32 * WP2_MAX_WARPS, 1) scan_fwd_wp2_kernel(const zg_scan_params p) {
     extern __shared__ __align__(1024) unsigned char smem_all[];
     const int lane = threadIdx.x & 31;
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
@@ -265,16 +265,15 @@ __global__ void __launch_bounds__(32 * WP2_MAX_WARPS, 2) scan_fwd_wp2_kernel(con
     wp2_body<T, PLAIN>(p, smem_all + warp * Wp2Layout::WARP_BYTES, lane, wu / units, unit / units_per_group, unit * WP2_CH);
 }
 
-// CTA shape.  The warps exchange nothing, so the CTA size is free; what it decides is how the SM's warp schedulers treat the warps:
-// they favour the oldest warps, which finish early, and the youngest run the tail with too few peers to keep the MUFU pipe busy.
-// When the whole problem fits one wave, the warps of an SM are therefore packed into one or two large CTAs (with two, either of them
-// alone keeps the pipe busy while the other is starved); problems of several waves keep small CTAs (finished CTAs are replaced).
-// Up to 18 warps per SM (112 registers) in two CTAs.
+// CTA shape.  The warps exchange nothing, so the CTA size is free; what it decides is how the warps land on the SM's four
+// sub-partitions, each of which issues to its own MUFU pipe.  At 96 registers an SM holds 21 warps.  When the whole problem fits one
+// wave of at most 20 warps per SM, each SM gets its share as ONE CTA, whose warps spread evenly over the sub-partitions (config 2,
+// 2560 units on 132 SMs: 128 CTAs of 20 warps, 5 per sub-partition; H100 SXM 700 W: 0.509 ms, against 0.537 ms for two 10-warp CTAs
+// per SM and 0.644 ms for 854 three-warp CTAs, whose uneven packing leaves some sub-partitions with 6 warps).  Problems of several
+// waves keep three-warp CTAs, seven per SM (finished CTAs are replaced; 5, 10 and 20 warps measured no faster there).
 inline int wp2_pick_warps(long long units, int sms) {
-    if (units > 18LL * sms) return 3;                                        // several waves: six small CTAs per SM
-    const long long per_sm = (units + sms - 1) / sms;                        // warps on the fullest SM
-    const int ctas_per_sm = per_sm > 4 ? 2 : 1;
-    return (int)((units + (long long)sms * ctas_per_sm - 1) / ((long long)sms * ctas_per_sm));
+    if (units > (long long)WP2_MAX_WARPS * sms) return 3;
+    return (int)((units + sms - 1) / sms);
 }
 
 template <typename T, bool PLAIN> int wp2_launch(const zg_scan_params &p, cudaStream_t stream) {

@@ -55,16 +55,30 @@ def scan_hot_path_ok(dtype, E, L, N, R):
 
 
 def block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, final=False, mod_div=1, want_modded=True, want_rstd=False,
-               mix_bcast=False, path_scale=None):
+               mix_bcast=False, path_scale=None, x_from=None):
     """zg_block_tail_fwd wrapper.  x: (Bt, L, D) contiguous; gate/shift/scale: (Bt // mod_div, D)
     views with a common row stride.  Returns residual_out (fp32), normed, modded.
     mix_bcast: ``mix`` is one (L, D) table added to every batch element (gate None = 1): the positional embedding.
-    path_scale: (Bt,) drop-path multipliers in x.dtype (zg_block_tail_fwd_dp): hidden * path_scale[b] joins the residual."""
+    path_scale: (Bt,) drop-path multipliers in x.dtype (zg_block_tail_fwd_dp): hidden * path_scale[b] joins the residual.
+    x_from = (rstd, norm_w) of the previous tail, norm_w in the activation dtype, with x None (zg_block_tail_fwd_rebuild): x is that
+    tail's normed output, rebuilt from `residual` (its residual_out) in the kernel; normed is then only written (and returned) when
+    final."""
     _lib.require_cuda(x, mix, gate, shift, scale, norm_w, residual, rowmap, path_scale)
-    if path_scale is not None and (path_scale.dtype != x.dtype or tuple(path_scale.shape) != (x.shape[0],) or not path_scale.is_contiguous()):
-        raise RuntimeError(f"block_tail: path_scale must be a contiguous ({x.shape[0]},) tensor in {x.dtype}, got "
+    if (x is None) != (x_from is not None) or (x_from is not None and (residual is None or path_scale is not None or mix_bcast)):
+        raise RuntimeError("block_tail: x_from replaces x, needs the residual and takes no path_scale / mix_bcast")
+    if x_from is not None:
+        x_rstd, x_norm_w = x_from
+        _lib.require_cuda(x_rstd, x_norm_w)
+        xdt, xdev = x_norm_w.dtype, residual.device
+        Bt, L, D = residual.shape
+        if x_rstd.dtype != torch.float32 or x_rstd.numel() != Bt * L or not x_rstd.is_contiguous() or x_norm_w.numel() != D:
+            raise RuntimeError("block_tail: x_from needs the previous tail's (Bt * L,) fp32 rstd and its (D,) norm_w")
+    else:
+        xdt, xdev = x.dtype, x.device
+        Bt, L, D = x.shape
+    if path_scale is not None and (path_scale.dtype != xdt or tuple(path_scale.shape) != (Bt,) or not path_scale.is_contiguous()):
+        raise RuntimeError(f"block_tail: path_scale must be a contiguous ({Bt},) tensor in {xdt}, got "
                            f"{tuple(path_scale.shape)} {path_scale.dtype}")
-    Bt, L, D = x.shape
     if mod_div != 1:
         # modulation vectors are per ORIGINAL batch element; expand to the folded batch (tiny)
         gate = None if gate is None else gate.repeat_interleave(mod_div, dim=0)
@@ -75,20 +89,20 @@ def block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, final=
     for m in mods:
         if m.stride(0) != rs or m.stride(1) != 1:
             raise RuntimeError("block_tail: modulation views must share one row stride")
-    if norm_w.dtype != x.dtype:
-        norm_w = norm_w.to(x.dtype)
+    if norm_w.dtype != xdt:
+        norm_w = norm_w.to(xdt)
     # the kernel reads every operand with ONE dtype (x's).  Under bf16 autocast with fp32 master weights the tokens can be
     # fp32 (embed() adds an fp32 pos_embed) while the adaLN chunks and the mixer output are bf16: bring them to x.dtype
     # instead of letting the kernel reinterpret the buffers.
     def _as_x(t):
-        return t if (t is None or t.dtype == x.dtype) else t.to(x.dtype)
+        return t if (t is None or t.dtype == xdt) else t.to(xdt)
     mix = _as_x(mix)
     if mix is not None and not mix.is_contiguous():
         mix = mix.contiguous()
-    if any(m is not None and m.dtype != x.dtype for m in (gate, shift, scale)):
+    if any(m is not None and m.dtype != xdt for m in (gate, shift, scale)):
         # re-materialise the three views in x.dtype with one common row stride
-        D_ = x.shape[-1]
-        packed = torch.zeros((x.shape[0] // mod_div if mod_div != 1 else x.shape[0], 3 * D_), dtype=x.dtype, device=x.device)
+        D_ = D
+        packed = torch.zeros((Bt // mod_div if mod_div != 1 else Bt, 3 * D_), dtype=xdt, device=xdev)
         for i_, m in enumerate((gate, shift, scale)):
             if m is not None:
                 packed[:, i_ * D_:(i_ + 1) * D_] = m
@@ -97,21 +111,23 @@ def block_tail(x, mix, gate, shift, scale, norm_w, residual, rowmap, eps, final=
         scale = None if scale is None else packed[:, 2 * D_:]
     if residual is not None and residual.dtype != torch.float32:
         raise RuntimeError("block_tail: the residual stream must be fp32 (residual_in_fp32=True)")
-    res_out = torch.empty((Bt, L, D), dtype=torch.float32, device=x.device) if not final else None
-    normed = torch.empty_like(x)
-    modded = torch.empty_like(x) if (want_modded and not final) else None
+    res_out = torch.empty((Bt, L, D), dtype=torch.float32, device=xdev) if not final else None
+    normed = torch.empty((Bt, L, D), dtype=xdt, device=xdev) if (x_from is None or final) else None
+    modded = torch.empty((Bt, L, D), dtype=xdt, device=xdev) if (want_modded and not final) else None
     p = _lib.BlockTailParams()
     p.x, p.mix, p.gate, p.shift, p.scale = _lib.ptr(x), _lib.ptr(mix), _lib.ptr(gate), _lib.ptr(shift), _lib.ptr(scale)
     p.norm_w, p.residual, p.rowmap = _lib.ptr(norm_w), _lib.ptr(residual), _lib.ptr(rowmap)
     p.residual_out, p.normed, p.modded = _lib.ptr(res_out), _lib.ptr(normed), _lib.ptr(modded)
     p.mod_rs = rs
     p.batch, p.seqlen, p.dim = Bt, L, D
-    p.dtype, p.final_layer, p.eps = _lib.dt(x), int(final), float(eps)
-    rstd = torch.empty((Bt * L,), dtype=torch.float32, device=x.device) if want_rstd else None
+    p.dtype, p.final_layer, p.eps = _lib.dt(xdt), int(final), float(eps)
+    rstd = torch.empty((Bt * L,), dtype=torch.float32, device=xdev) if want_rstd else None
     p.rstd = _lib.ptr(rstd)
     if mix_bcast and (mix is None or mix.numel() != L * D or gate is not None or rowmap is not None or residual is not None):
         raise RuntimeError("block_tail: mix_bcast takes a (seqlen, dim) mix table and no gate / rowmap / residual")
-    if path_scale is not None:
+    if x_from is not None:
+        _lib.call("zg_block_tail_fwd_rebuild", _lib.BlockTailRebuildParams(p, _lib.ptr(x_rstd), _lib.ptr(x_norm_w)))
+    elif path_scale is not None:
         _lib.call("zg_block_tail_fwd_dp", _lib.BlockTailDpParams(p, _lib.ptr(path_scale)))
     else:
         _lib.call("zg_block_tail_fwd_pe" if mix_bcast else "zg_block_tail_fwd", p)
@@ -364,8 +380,13 @@ class ZigMaEngine:
         mods = _linear(F.silu(c), self.ada_w, self.ada_b).view(B, depth, nmod, D)  # shift, scale, gate per block (one GEMM for all)
         eps = m.blocks[0].norm.eps
         lay0 = self.layers[0]
-        residual, normed, modded = block_tail(hs, pe, None, mods[:, 0, 0], mods[:, 0, 1], lay0["norm_w"], None, None, eps,
-                                              mix_bcast=pe is not None)
+        # below the first tail, each tail rebuilds its x (the previous tail's normed output) from the residual row it reads anyway
+        # and the previous tail's rstd and norm_w, so normed is not written and read back between tails.  Not for text blocks:
+        # their prologue reads normed.
+        rebuild = not m.has_text and D <= 1024
+        residual, normed, modded, *rstd = block_tail(hs, pe, None, mods[:, 0, 0], mods[:, 0, 1], lay0["norm_w"], None, None, eps,
+                                                     mix_bcast=pe is not None, want_rstd=rebuild)
+        prev_w = lay0["norm_w"]
         for i, lay in enumerate(self.layers):
             mix, rowmap, fold = self._mixer(modded, lay)
             last = i == depth - 1
@@ -387,15 +408,19 @@ class ZigMaEngine:
                                              rowmap, blk.norm_msa.eps, mod_div=fold)
                 fold = 1
                 mix, rowmap, gate, normed = blk.msa(q_in.view(B, L, D), text=text, mask=None).contiguous(), None, mods[:, i, 5], hidden.view(B, L, D)
+            tail_x = dict(x_from=(rstd[0], prev_w.to(hs.dtype)), want_rstd=not last) if rebuild else {}
             if fold != 1:     # spatial video layer: rows are (b t, k); same memory as (b, t k)
                 Bf = B * fold
-                residual, normed, modded = block_tail(normed.view(Bf, L // fold, D), mix, gate, shift, scale, nw,
-                                                      residual.view(Bf, L // fold, D), rowmap, neps, final=last, mod_div=fold)
-                normed = normed.view(B, L, D)
+                residual, normed, modded, *rstd = block_tail(None if rebuild else normed.view(Bf, L // fold, D), mix, gate, shift, scale,
+                                                             nw, residual.view(Bf, L // fold, D), rowmap, neps, final=last, mod_div=fold,
+                                                             **tail_x)
+                normed = normed.view(B, L, D) if normed is not None else None
                 if not last:
                     residual, modded = residual.view(B, L, D), modded.view(B, L, D)
             else:
-                residual, normed, modded = block_tail(normed, mix, gate, shift, scale, nw, residual, rowmap, neps, final=last)
+                residual, normed, modded, *rstd = block_tail(None if rebuild else normed, mix, gate, shift, scale, nw, residual, rowmap,
+                                                             neps, final=last, **tail_x)
+            prev_w = nw
         out = _linear(normed.reshape(B * L, D), m.final_layer.linear.weight, m.final_layer.linear.bias).view(B, L, -1)   # un-embed
         if m.video_frames > 0:
             return m.unpatchify_video(out, m.video_frames)
