@@ -396,7 +396,8 @@ int zg_cross_attn_bwd(const zg_xattn_bwd_params *p, void *workspace, int64_t wor
  * C row-major ldc.  out_rowmap (int32[rows_per_batch] or NULL): output row m of batch
  * m / rows_per_batch is stored at row out_rowmap[m % rows_per_batch] of that batch (scatter of
  * the out_proj result back to raster order, mamba_simple.py:388-394).
- * Any M, N, K >= 1 with lda/ldb/ldc multiples of 8 (remainders come from TMA zero fill / clipped stores).  The CUtensorMaps are built on the host per call and passed to the
+ * Any M, N, K >= 1 with lda/ldb/ldc multiples of 8 (remainders come from TMA zero fill / clipped stores); nothing of C outside
+ * its M x N window is written, so C may be a window of a wider matrix.  The CUtensorMaps are built on the host per call and passed to the
  * kernel by value (__grid_constant__), so nothing has to outlive the call.
  */
 typedef struct {
@@ -408,6 +409,10 @@ typedef struct {
 } zg_gemm_params;
 
 int zg_gemm_bf16_tn(const zg_gemm_params *p, void *stream);
+/* The kernel zg_gemm_bf16_tn launches for an M x N output (host arithmetic only, no GPU needed): tile width *bn (64, 80, 128, 160,
+ * 256) and cluster size *cl (1, 2, 4), after the ZG_GEMM_BN / ZG_GEMM_CLUSTER overrides (read on every call) and the halving of
+ * the cluster.  Returns 0, or nonzero for M or N < 1. */
+int zg_gemm_kernel_choice(int32_t M, int32_t N, int32_t *bn, int32_t *cl);
 
 
 /* ---------------------------------------------------------------------------------------------

@@ -22,7 +22,7 @@ def _declared():
 def test_header_declares_entry_points():
     names = _declared()
     for n in ("zg_selective_scan_fwd", "zg_selective_scan_bwd", "zg_causal_conv1d_fwd", "zg_causal_conv1d_bwd",
-              "zg_add_norm_fwd", "zg_add_norm_bwd", "zg_block_tail_fwd", "zg_block_tail_bwd", "zg_gemm_bf16_tn",
+              "zg_add_norm_fwd", "zg_add_norm_bwd", "zg_block_tail_fwd", "zg_block_tail_bwd", "zg_gemm_bf16_tn", "zg_gemm_kernel_choice",
               "zg_adamw_ema_step", "zg_last_error"):
         assert n in names
 

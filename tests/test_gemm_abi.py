@@ -40,8 +40,10 @@ def _gemm_functions():
 
 def test_sass_gemm_main_loop_has_no_gpu_scope_fence():
     funcs = _gemm_functions()
-    # every tile width the dispatcher picks, each with clusters of 1, 2 and 4 CTAs
-    assert {(bn, cl) for bn in ("64", "80", "128", "160", "256") for cl in ("1", "2", "4")} <= {k[:2] for k in funcs}, sorted(funcs)
+    # every tile width the dispatcher picks, each with clusters of 1, 2 and 4 CTAs, except 80-wide tiles in clusters of 4 (a CTA's
+    # 20-row multicast slice of the weight tile would not be whole 8-row swizzle groups)
+    want = {(bn, cl) for bn in ("64", "80", "128", "160", "256") for cl in ("1", "2", "4")} - {("80", "4")}
+    assert want == {k[:2] for k in funcs}, sorted(funcs)
     clustered_fences = 0
     for args, lines in funcs.items():
         mma = [i for i, l in enumerate(lines) if "HGMMA" in l]

@@ -141,6 +141,7 @@ DET_OPS = ["zg_selective_scan_bwd", "zg_causal_conv1d_bwd", "zg_add_norm_bwd", "
 EXPORTS += [n + s for n in DET_OPS for s in ("_det", "_det_workspace_bytes")]
 # cross-attention (always atomic-free, so no _det twin); the last two have signatures of their own
 EXPORTS += ["zg_cross_attn_fwd", "zg_cross_attn_bwd", "zg_cross_attn_bwd_workspace_bytes"]
+EXPORTS += ["zg_gemm_kernel_choice"]
 
 _lib = None
 
@@ -173,6 +174,7 @@ def lib():
         l.zg_cross_attn_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
         l.zg_cross_attn_bwd_workspace_bytes.restype = C.c_int64
         l.zg_cross_attn_bwd_workspace_bytes.argtypes = [C.c_void_p]
+        l.zg_gemm_kernel_choice.argtypes = [C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         _lib = l
     return _lib
 
@@ -186,6 +188,15 @@ def scan_kernel_choice(batch, dim, sms=132, training_forward=False):
     nd, ns = C.c_int32(0), C.c_int32(0)
     mode = lib().zg_scan_kernel_choice(int(batch) * (int(dim) // 16), int(sms), int(bool(training_forward)), C.byref(nd), C.byref(ns))
     return int(mode), int(nd.value), int(ns.value)
+
+
+def gemm_kernel_choice(M, N):
+    """(tile width, cluster size) of the zg::gemm_bf16_tn_kernel instantiation that zg_gemm_bf16_tn launches for an M x N output
+    (zg_gemm_kernel_choice; host arithmetic, with the ZG_GEMM_BN / ZG_GEMM_CLUSTER overrides of the current environment)."""
+    bn, cl = C.c_int32(0), C.c_int32(0)
+    if lib().zg_gemm_kernel_choice(int(M), int(N), C.byref(bn), C.byref(cl)) != 0:
+        raise RuntimeError(f"zg_gemm_kernel_choice: {lib().zg_last_error().decode()}")
+    return int(bn.value), int(cl.value)
 
 
 def last_scan_kernel():

@@ -251,7 +251,7 @@ struct GemmArgs {
     const int32_t *out_rowmap;
     int64_t ldc;
     int M, N, K, rows_per_batch;
-    int tma_store;      // 1: epilogue goes through smem + TMA store (needs 16-byte aligned C rows)
+    int tma_store;      // 1: epilogue goes through smem + TMA store (needs 16-byte aligned C rows and N % 8 == 0)
 };
 
 template <int BN, int CL>
@@ -478,7 +478,10 @@ template <int BN, int CL> static int launch_gemm(const zg_gemm_params &p, cudaSt
     CUtensorMap tmA, tmB, tmC;
     if (int rc = make_map(&tmA, p.A, p.M, p.K, p.lda, G_BM)) return rc;
     if (int rc = make_map(&tmB, p.B, p.N, p.K, p.ldb, BN / CL)) return rc;
-    const bool tma_store_ok = !p.out_rowmap && p.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(p.C) & 15) == 0;
+    // TMA store: 16-byte aligned C rows, and N a multiple of 8 -- clipped at a column N inside a 16-byte unit, the store also writes
+    // the rest of that unit (measured on H100: columns N .. round8(N) - 1 of every row, i.e. outside C when C is a window of a wider
+    // matrix), so such calls leave by direct stores
+    const bool tma_store_ok = !p.out_rowmap && p.N % 8 == 0 && p.ldc % 8 == 0 && (reinterpret_cast<uintptr_t>(p.C) & 15) == 0;
     if (tma_store_ok) {
         if (int rc = make_map(&tmC, p.C, p.M, p.N, p.ldc, 16, false)) return rc;
     } else {
@@ -525,22 +528,38 @@ template <int BN, int CL> static int launch_gemm(const zg_gemm_params &p, cudaSt
     return zg_check_launch("gemm_bf16_tn");
 }
 
-// cluster size: ZG_GEMM_CLUSTER = 1 | 2 | 4 (default 2 when the problem has at least that many row tiles)
-static int gemm_cluster_setting() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("ZG_GEMM_CLUSTER");
-        v = e ? atoi(e) : 2;
-        if (v != 1 && v != 2 && v != 4) v = 2;
+// Tile width and cluster size of an M x N call.  Width: ZG_GEMM_BN = 64 | 80 | 128 | 160 | 256 forces it; otherwise, among
+// {256, 160, 128, 80, 64}, the WIDEST whose ragged last column tile wastes <= 5 % of the MMA work, else the one that wastes least
+// (wider tiles move fewer operand bytes per MAC through L2 and re-read A fewer times).  160 exists for N = 640 (out_proj of the
+// D = 640 models: 4 x 160 exactly; 256-wide tiles pad it to 768 = 17 % idle MMAs), 80 for the x_proj widths 72 / 80 (one pass over A
+// instead of two 64-wide ones).  Cluster: ZG_GEMM_CLUSTER = 1 | 2 | 4 (default 2), halved while the problem has fewer row tiles than
+// the cluster has CTAs or a CTA's multicast slice of the weight tile would not be whole 8-row swizzle groups (so never 4 with
+// width 80).  Both settings are read on every call, so one process can run every instantiation.
+static void gemm_choice(int M, int N, int &bn, int &cl) {
+    const char *be = getenv("ZG_GEMM_BN"), *ce = getenv("ZG_GEMM_CLUSTER");
+    bn = be ? atoi(be) : 0;
+    if (bn != 64 && bn != 80 && bn != 128 && bn != 160 && bn != 256) {
+        const int cand[5] = {256, 160, 128, 80, 64};
+        auto waste = [&](int b) { return (double)(((N + b - 1) / b) * b - N) / (double)(((N + b - 1) / b) * b); };
+        bn = 0;
+        for (int i = 0; i < 5 && !bn; ++i)
+            if (waste(cand[i]) <= 0.05) bn = cand[i];
+        if (!bn) {
+            bn = 64;
+            for (int i = 0; i < 5; ++i)
+                if (waste(cand[i]) < waste(bn) - 1e-9) bn = cand[i];
+        }
     }
-    return v;
+    cl = ce ? atoi(ce) : 2;
+    if (cl != 1 && cl != 2 && cl != 4) cl = 2;
+    const int m_tiles = (M + G_BM - 1) / G_BM;
+    while (cl > 1 && (m_tiles < cl || (bn / cl) % 8 != 0)) cl >>= 1;
 }
 
-template <int BN> static int launch_gemm_cl(const zg_gemm_params &p, cudaStream_t s) {
-    int cl = gemm_cluster_setting();
-    const int m_tiles = (p.M + G_BM - 1) / G_BM;
-    while (cl > 1 && (m_tiles < cl || (BN / cl) % 8 != 0)) cl >>= 1;     // (a CTA's multicast slice must be whole 8-row swizzle groups)
-    if (cl == 4) return launch_gemm<BN, 4>(p, s);
+template <int BN> static int launch_gemm_cl(const zg_gemm_params &p, int cl, cudaStream_t s) {
+    if constexpr ((BN / 4) % 8 == 0) {        // (gemm_choice never asks for the others)
+        if (cl == 4) return launch_gemm<BN, 4>(p, s);
+    }
     if (cl == 2) return launch_gemm<BN, 2>(p, s);
     return launch_gemm<BN, 1>(p, s);
 }
@@ -556,28 +575,20 @@ extern "C" int zg_gemm_bf16_tn(const zg_gemm_params *pp, void *stream) {
     ZG_REQUIRE((reinterpret_cast<uintptr_t>(p.A) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.B) & 15) == 0, "gemm_bf16_tn: A and B must be 16-byte aligned");
     ZG_REQUIRE(!p.out_rowmap || (p.rows_per_batch > 0 && p.M % p.rows_per_batch == 0), "gemm_bf16_tn: out_rowmap needs rows_per_batch dividing M");
     cudaStream_t s = (cudaStream_t)stream;
-    // tile width: among {256, 160, 128, 80, 64} the WIDEST whose ragged last column tile wastes <= 5 % of the MMA work, else the
-    // one that wastes least (wider tiles move fewer operand bytes per MAC through L2 and re-read A fewer times).  160 exists for
-    // N = 640 (out_proj of the D = 640 models: 4 x 160 exactly; 256-wide tiles pad it to 768 = 17 % idle MMAs), 80 for the
-    // x_proj widths 72 / 80 (one pass over A instead of two 64-wide ones).
-    static int bn_env = -1;
-    if (bn_env < 0) { const char *e = getenv("ZG_GEMM_BN"); bn_env = e ? atoi(e) : 0; }
-    int bn = bn_env;
-    if (bn != 64 && bn != 80 && bn != 128 && bn != 160 && bn != 256) {
-        const int cand[5] = {256, 160, 128, 80, 64};
-        auto waste = [&](int b) { return (double)(((p.N + b - 1) / b) * b - p.N) / (double)(((p.N + b - 1) / b) * b); };
-        bn = 0;
-        for (int i = 0; i < 5 && !bn; ++i)
-            if (waste(cand[i]) <= 0.05) bn = cand[i];
-        if (!bn) {
-            bn = 64;
-            for (int i = 0; i < 5; ++i)
-                if (waste(cand[i]) < waste(bn) - 1e-9) bn = cand[i];
-        }
-    }
-    if (bn == 256) return zg::launch_gemm_cl<256>(p, s);
-    if (bn == 160) return zg::launch_gemm_cl<160>(p, s);
-    if (bn == 128) return zg::launch_gemm_cl<128>(p, s);
-    if (bn == 80) return zg::launch_gemm_cl<80>(p, s);
-    return zg::launch_gemm_cl<64>(p, s);
+    int bn = 0, cl = 0;
+    zg::gemm_choice(p.M, p.N, bn, cl);
+    if (bn == 256) return zg::launch_gemm_cl<256>(p, cl, s);
+    if (bn == 160) return zg::launch_gemm_cl<160>(p, cl, s);
+    if (bn == 128) return zg::launch_gemm_cl<128>(p, cl, s);
+    if (bn == 80) return zg::launch_gemm_cl<80>(p, cl, s);
+    return zg::launch_gemm_cl<64>(p, cl, s);
+}
+
+extern "C" int zg_gemm_kernel_choice(int32_t M, int32_t N, int32_t *bn, int32_t *cl) {
+    ZG_REQUIRE(M > 0 && N > 0, "gemm_kernel_choice: bad shape (%d, %d)", M, N);
+    int b = 0, c = 0;
+    zg::gemm_choice(M, N, b, c);
+    if (bn) *bn = b;
+    if (cl) *cl = c;
+    return 0;
 }
